@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """HVP-iters/sec of the hypergradient K-loop (BASELINE.json metric).
 
-    python bench.py [--gpus N --steps K --warmup W] [--workload NAME] [--impl reference]
+    python bench.py [--gpus N --steps K --warmup W] [--workload NAME] [--impl reference] [--dump-outputs DIR]
 
 One "step" = one full K-loop (K Hessian-vector products + the Neumann/CG vector updates) over one
 synthetic batch, inputs resident in HBM; prologue (lower forward + tape) is built once, outside the
@@ -14,6 +14,10 @@ K-loop, one all-reduce of the hypergradient in ``e2e``.
 ``--impl reference`` times the reference's own CPU autograd path (oracle/_ref, the unmodified reference mirrored by
 oracle/fetch_ref.sh; the oracle port if that mirror is missing) on the host cores.  The default run reports the
 config the >=60 % roofline target is quoted on (implicit_maml) and carries configs 2 and 5 as `extra` sub-records.
+
+``--dump-outputs DIR`` writes what the last timed step of the headline workload returned (the hypergradient, one
+array per parameter tensor) as ``DIR/<workload>.<index>.npy`` in float32; the workloads are seeded, so two builds run
+with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -40,7 +44,8 @@ WORKLOADS = {
 }
 DEFAULT = "implicit_maml"      # the config BASELINE.json's ">=60 % HBM roofline on the Neumann K=20 path" is quoted on
 EXTRA = ("learning_to_reweight", "bert_data_reweighting", "neural_architecture_search")   # sub-records of the default run
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024      # H100 SXM
+DUMP_MAX_BYTES = 64 * 1024 * 1024
 
 
 # -------------------------------------------------------------------------------------------------
@@ -99,8 +104,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), d.get("bf16_tflops_sustained", 1400.0), "measured"
-    return 6650.0, 1590.0, "fallback"
+        return d.get("hbm_gbs", 3350.0), d.get("bf16_tflops_sustained", 989.0), "measured"
+    return 3350.0, 989.0, "datasheet"      # H100 SXM: HBM3 bandwidth, dense BF16
 
 
 def flush_l2(buf):
@@ -108,6 +113,23 @@ def flush_l2(buf):
 
 
 # -------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, name, tensors):
+    """Write the arrays a caller of the timed path receives as float32 .npy files, at most DUMP_MAX_BYTES in all: above
+    that, every tensor contributes the same fraction of its elements, picked by a fixed seed."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    flat = [t.detach().reshape(-1).float().cpu() for t in tensors]
+    total = sum(f.numel() for f in flat)
+    keep = min(1.0, DUMP_MAX_BYTES / 4 / max(total, 1))
+    gen = torch.Generator().manual_seed(0)
+    for i, f in enumerate(flat):
+        if keep < 1.0:
+            idx = torch.randperm(f.numel(), generator=gen)[: max(1, int(f.numel() * keep))].sort().values
+            f = f[idx]
+        np.save(os.path.join(out_dir, f"{name}.{i:03d}.npy"), f.numpy().astype(np.float32))
+
+
 def build_workload(name, device, seed=0):
     from betty_b200 import workloads as W
 
@@ -205,7 +227,7 @@ def run_reference(args):
 
 
 # -------------------------------------------------------------------------------------------------
-def measure(name, args, dev, dist, world, rank, local, steps, e2e_steps, with_cpu):
+def measure(name, args, dev, dist, world, rank, local, steps, e2e_steps, with_cpu, dump_dir=None):
     """One workload: K-loop rate (inputs resident), e2e through the plugin call from pinned host buffers, roofline."""
     import gc
 
@@ -238,7 +260,7 @@ def measure(name, args, dev, dist, world, rank, local, steps, e2e_steps, with_cp
         K = kw["K"] = 1
     else:
         call = E.HypergradientCall(wl.lower, method)
-    flush = torch.zeros(L2_BYTES // 4 * 2, device=dev)  # 252 MB > L2, written between steps
+    flush = torch.zeros(L2_BYTES // 4 * 2, device=dev)  # twice the L2, written between steps
 
     for _ in range(args.warmup):
         call.solve(wl.vector)
@@ -250,15 +272,19 @@ def measure(name, args, dev, dist, world, rank, local, steps, e2e_steps, with_cp
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
     barrier()
     t0 = time.perf_counter()
+    out = None
     for i in range(steps):
         ev[i][0].record()
-        call.solve(wl.vector)
+        out = call.solve(wl.vector)
         ev[i][1].record()
         flush_l2(flush)
     barrier()
     wall = time.perf_counter() - t0
     sampler.stop_flag.set()
     sampler.join()
+    if dump_dir is not None and rank == 0 and out is not None:
+        dump_outputs(dump_dir, name, out)
+    del out
     step_ms = [a.elapsed_time(b) for a, b in ev]
     dev_ms = sum(step_ms)  # device time of the K steps, L2 flushes excluded
     launches = N.launch_counter - launches0
@@ -286,15 +312,6 @@ def measure(name, args, dev, dist, world, rank, local, steps, e2e_steps, with_cp
                              "note": "SURVEY 8(d) bytes x measured K-loop rate (vector kernels K1-K3 included in the time)"}
     elif method == "darts":
         roof = fd_kernel_roofline(wl, dev, hbm, which)
-    try:
-        with open(os.path.join(ROOT, "profiles", "traffic.json")) as f:
-            tr = json.load(f).get(name, {})
-        for key, rec in tr.items():
-            if roof and roof.get("kernel", "").startswith(key):
-                roof["traffic"] = rec["bytes"]
-                roof["traffic_source"] = rec["source"]
-    except (OSError, ValueError, KeyError):
-        pass
     n_params = call.layout.n_logical
     del call
     gc.collect()
@@ -346,7 +363,8 @@ def measure(name, args, dev, dist, world, rank, local, steps, e2e_steps, with_cp
         "value": value, "unit": "HVP-iters/s", "ms_per_step": ms_per_step, "steps": steps,
         "dtype": "f32" if wl.lower.config.precision == "fp32" else "bf16+f32",
         "config": {"workload": name, "describe": desc, "K": K, "method": method, "hvp": args.hvp,
-                   "cuda_graph": E.settings.cuda_graph, "l2": "252 MB buffer rewritten between timed steps",
+                   "cuda_graph": E.settings.cuda_graph,
+                   "l2": f"{2 * L2_BYTES >> 20} MB buffer rewritten between timed steps",
                    "parallelism": f"replicas x{world} (local solve per rank, SURVEY 8e)",
                    "n_params": n_params, "wall_s": wall},
         "clocks": sampler.summary(),
@@ -411,6 +429,8 @@ def main():
     ap.add_argument("--ref-budget-s", type=float, default=60.0, help="--impl reference: CPU seconds of timed K-loop")
     ap.add_argument("--cpu-budget-s", type=float, default=12.0, help="cpu_baseline leg: CPU seconds of timed K-loop")
     ap.add_argument("--e2e-steps", type=int, default=5)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the headline workload's last timed output as DIR/<workload>.<i>.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     extras = [] if (args.workload is not None or args.no_extra) else list(EXTRA)
@@ -439,7 +459,8 @@ def main():
     E.settings.hvp = args.hvp
     E.settings.cuda_graph = not args.no_graph
     with_cpu = rank == 0 and world == 1 and not args.no_cpu_baseline
-    main_rec = measure(args.workload, args, dev, dist, world, rank, local, args.steps, args.e2e_steps, with_cpu)
+    main_rec = measure(args.workload, args, dev, dist, world, rank, local, args.steps, args.e2e_steps, with_cpu,
+                       dump_dir=args.dump_outputs)
     line = {
         "metric": "HVP-iters/sec", "value": main_rec["value"], "unit": "HVP-iters/s", "n_gpus": world,
         "steps": args.steps, "warmup": args.warmup, "ms_per_step": main_rec["ms_per_step"], "higher_is_better": True,

@@ -1,4 +1,4 @@
-"""betty_b200 -- B200-native hypergradient engine behind ``betty.hypergradient.{neumann, cg, darts}``."""
+"""betty_b200 -- H100-native hypergradient engine behind ``betty.hypergradient.{neumann, cg, darts}``."""
 from . import hypergradient  # noqa: F401
 from .hypergradient import install  # noqa: F401
 

@@ -85,11 +85,11 @@ def sources():
 
 
 def build(verbose: bool = False) -> str:
-    """Compile every ``csrc/*.cu`` for sm_100a into ``libbetty_b200.so`` (in-tree, so it travels to the
+    """Compile every ``csrc/*.cu`` for sm_90a into ``libbetty_b200.so`` (in-tree, so it travels to the
     GPU box with the snapshot).  Incremental: one object per source, rebuilt when older than its
     source or any header."""
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    flags = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler",
+    flags = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler",
              "-fPIC", "-I", INCLUDE]
     hdrs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     hdrs.append(os.path.join(INCLUDE, "betty_b200.h"))
@@ -157,4 +157,4 @@ def require_cuda():
     import torch
 
     if not torch.cuda.is_available():
-        raise NativeError("betty_b200 needs a CUDA device (sm_100a); there is no CPU fallback.")
+        raise NativeError("betty_b200 needs a CUDA device (sm_90a); there is no CPU fallback.")

@@ -1,4 +1,4 @@
-// Shared device helpers for the betty_b200 sm_100a kernels.
+// Shared device helpers for the betty_b200 sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -9,7 +9,7 @@
 #define BB_ERR_ARG (-1)
 #define BB_ERR_UNSUPPORTED (-2)
 
-#define BB_SM_COUNT 148  // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+#define BB_SM_COUNT 132  // H100 SXM; grids are sized in multiples of this
 
 #define BB_CUDA_TRY(expr)                 \
   do {                                    \

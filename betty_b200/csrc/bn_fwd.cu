@@ -2,10 +2,8 @@
 //
 // The prologue of every plugin call runs the user's lower forward once (reference neumann.py:31, cg.py:27).  On a
 // channels-first activation of 64 channels PyTorch's `batch_norm_collect_statistics_kernel` launches one block per
-// channel (64 blocks on 148 SMs, strided bf16 reads): 5.4 ms for 800 x 64 x 84 x 84 bf16 (profiles/
-// r02_launches_maml_final.csv, ids 9 / 21 / 33 / 45: 7.6 ms of the 13 ms forward).  When asked to
-// (BB200_PROLOGUE_BN_MIN, opt-in: see profiles/r02_prologue_bn.md for why bit-identical base activations matter for the
-// bf16 parity bar) the dispatch-mode recorder (betty_b200/trace.py) executes aten.native_batch_norm(training=True) on
+// channel (64 blocks for the whole GPU, strided bf16 reads).  When asked to (BB200_PROLOGUE_BN_MIN, opt-in: see
+// betty_b200/trace.py for why bit-identical base activations matter for the bf16 parity bar) the dispatch-mode recorder (betty_b200/trace.py) executes aten.native_batch_norm(training=True) on
 // large CUDA inputs with these three kernels instead -- same outputs (out, save_mean, save_invstd), same formula
 //     out = gamma * (x - mean) * invstd + beta,   invstd = rsqrt(biased_var + eps)
 // with the statistics reduced in fp64 in a fixed order (bit-reproducible run to run):
@@ -15,7 +13,7 @@
 //   bn_fwd_finalize_kernel one thread per channel adds the S partials in order -> mean, invstd, unbiased variance
 //   bn_fwd_apply_kernel    one pass: 16-byte loads / stores over the N*C planes
 //
-// HBM bound: x read twice, out written once (the second read of a 126 MB-L2-sized tensor partly hits L2).
+// HBM bound: x read twice, out written once (the second read partly hits L2 when the tensor is not much larger).
 #include "../../include/betty_b200.h"
 #include "bb_common.cuh"
 

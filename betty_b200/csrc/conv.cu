@@ -4,7 +4,7 @@
 //   TF  t_y  = conv(t_x, W) + conv(x, t_W) (+ t_b)                         C[o][p]     K = C*KH*KW
 //   BB  a_x  = dgrad(a_y, W)                                              C[c][p_in]  K = O*KH*KW
 //   TB  at_x = dgrad(at_y, W) + dgrad(a_y, t_W)
-//       at_W = wgrad(at_y, x) + wgrad(a_y, t_x)   (split-K, atomics)      C[o][cij]   K = N*HO*WO
+//       at_W = wgrad(at_y, x) + wgrad(a_y, t_x)   (split-K, fixed order)  C[o][cij]   K = N*HO*WO
 //       at_b = sum_{n,y,x} at_y
 // (SURVEY.md Appendix B "Conv2d".)  Spec: oracle/plan_interp.py tf_conv2d/bb_conv2d/tb_conv2d.
 #include <stdlib.h>
@@ -13,6 +13,7 @@
 #include "conv_small.h"
 #include "conv_tma.h"
 #include "gemm_tma.h"
+#include "tma.h"
 #include "gemm_tc.h"
 #include "plan.h"
 #include "tile_gemm.cuh"
@@ -123,16 +124,19 @@ struct PlaneStore {
 template <class LA, class LB, class SC>
 int launch(const LA& la, const LB& lb, const SC& sc, int64_t M, int64_t N, int64_t K, int npairs, int ksplit,
            cudaStream_t s) {
+  // ksplit > 1: partials in the plan's reduction workspace, summed in split order (tile_gemm.cuh splitk_reduce)
+  ksplit = bb_reduce_ws_splits(ksplit, sizeof(float) * M * N);
+  float* part = ksplit > 1 ? bb_reduce_ws.base : nullptr;
   if (M <= 16) {
     dim3 grid((unsigned)((N + 63) / 64), (unsigned)((M + 15) / 16), (unsigned)ksplit);
-    bb::tile_gemm_kernel<16, 64, 16, 1, 4, LA, LB, SC><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit);
+    bb::tile_gemm_kernel<16, 64, 16, 1, 4, LA, LB, SC><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit, part);
   } else {
     dim3 grid((unsigned)((N + 63) / 64), (unsigned)((M + 63) / 64), (unsigned)ksplit);
-    bb::tile_gemm_kernel<64, 64, 16, 4, 4, LA, LB, SC><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit);
+    bb::tile_gemm_kernel<64, 64, 16, 4, 4, LA, LB, SC><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit, part);
   }
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
-  return BB_OK;
+  return bb::splitk_reduce(sc, part, M, N, 1, ksplit, s);
 }
 
 // out[ch] += sum_{img, q} g[(img*CH + ch)*HW + q]
@@ -185,7 +189,7 @@ __global__ void __launch_bounds__(256) chansum_kernel(const float* __restrict__ 
   if (threadIdx.x == 0) atomicAdd(out + ch, acc);
 }
 
-// ---- tensor-core (tcgen05) implicit-GEMM operands, bf16-autocast graphs with >= 32 channels ----------
+// ---- tensor-core (wgmma) implicit-GEMM operands, bf16-autocast graphs with >= 32 channels ----------
 TcSrc pixrow(const void* p, int dt, int CH, int H, int W, const Geom& g, int GH, int GW, int flip) {
   TcSrc s{};
   s.p = p; s.dt = dt; s.mode = TC_PIXROW;
@@ -325,7 +329,7 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     if (rc) return rc;
   }
   if ((need & 2) && tc && nd.beta[1]) {
-    // D[(c,i,j)][o] = sum_pixels im2col(x)[cij][pixel] * at_y[o][pixel]  (+ t_x with a_y); split-K, atomics
+    // D[(c,i,j)][o] = sum_pixels im2col(x)[cij][pixel] * at_y[o][pixel]  (+ t_x with a_y); split-K, fixed-order reduce
     TcGemmArgs G{};
     G.M = CKK; G.N = g.O; G.K = P;
     int np = 0;
@@ -370,10 +374,6 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     int ksplit = (int)(want < maxs ? want : maxs);
     if (ksplit < 1) ksplit = 1;
     if (ksplit > 1024) ksplit = 1024;
-    if (ksplit > 1 && !nd.beta[1]) {
-      BB_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * g.O * CKK, s));
-      bb_launch_tally += 1;
-    }
     bb::StridedStore sc{out, CKK, 1, 0, nd.beta[1], nullptr, 0};
     rc = launch(la, lb, sc, g.O, CKK, P, np, ksplit, s);
     if (rc) return rc;

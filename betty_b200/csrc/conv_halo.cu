@@ -1,24 +1,22 @@
-// Halo-resident implicit-GEMM 3x3 convolution on tcgen05 (64 -> 64 channels, stride 1, padding 1), forward and
-// input-gradient form, up to two operand pairs accumulated into one TMEM tile:
+// Halo-resident implicit-GEMM 3x3 convolution on wgmma (64 -> 64 channels, stride 1, padding 1), forward and
+// input-gradient form, up to two operand pairs accumulated into one register tile:
 //
 //     out[img][n][y][x] (beta)= sum_pairs sum_(tap, ch) A_p[img][y + dy(tap)][x + dx(tap)][ch] * B_p[n][tap][ch]  (+ bias[n])
 //
 // gemm_tma_kernel's TMA_CONV mode brings one 128-pixel x 64-channel box per TAP into shared memory: nine shifted
-// copies of (almost) the same pixels per tile, 24 KB of shared-memory fill per 2.1 MFLOP.  ncu shows that kernel --
-// and cuDNN's own sm100 implicit-GEMM fprop, 127 us for the 42x42 layer = 0.82 PFLOP/s -- bound by that fill rate
-// (tensor pipe 22 %, profiles/r01_persist_ncu.md), not by the tensor cores.  Here the activation lives in a PADDED
-// NHWC layout  [N][H+2][W+2][64]  (zero border), i.e. one long matrix of 128-byte pixel rows in which a tap
-// displacement (dy, dx) is the constant row offset dy*(W+2) + dx.  A tile is 128 consecutive pixel rows; ONE TMA box of
-// 128 + 2(W+2) + 2 rows is loaded per (tile, pair) and the nine taps are nine UMMA descriptors pointing at different
-// 128-byte row offsets inside that band (SWIZZLE_128B is a function of the shared-memory address bits alone, so a
-// descriptor may start on any 128-byte row of a 1024-byte-aligned band; base-offset field 0, verified on B200).  The 2 x 9 weight tiles (144 KB) are loaded once per
-// CTA and stay resident.  Shared-memory fill per tile: 2 x 28 KB instead of 2 x 9 x 24 KB -> the MMA issue rate, not
-// the fill, bounds the kernel.  Rows that fall on the zero border compute garbage-free zeros' neighbours and are
-// simply not stored.
+// copies of (almost) the same pixels per tile, 24 KB of shared-memory fill per 2.1 MFLOP, which bounds that kernel
+// by the fill rate rather than by the tensor cores.  Here the activation lives in a PADDED NHWC layout
+// [N][H+2][W+2][64] (zero border), i.e. one long matrix of 128-byte pixel rows in which a tap displacement (dy, dx)
+// is the constant row offset dy*(W+2) + dx.  A tile is 128 consecutive pixel rows; ONE TMA box of 128 + 2(W+2) + 2
+// rows is loaded per (tile, pair) and the nine taps are nine wgmma descriptors pointing at different 128-byte row
+// offsets inside that band (SWIZZLE_128B is a function of the shared-memory address bits alone, so a descriptor may
+// start on any 128-byte row of a 1024-byte-aligned band with base offset 0).  The 2 x 9 weight tiles (144 KB) are
+// loaded once per CTA and stay resident.  Shared-memory fill per tile: 2 x 28 KB instead of 2 x 9 x 24 KB.  Rows that
+// fall on the zero border compute garbage-free zeros' neighbours and are simply not stored.
 //
-// Roles (192 threads, one CTA per SM, persistent over tiles): warp 0 = TMA producer, warp 1 = TMEM alloc + MMA issue,
-// warps 2-5 = epilogue (tcgen05.ld -> fp32 NCHW planes).  Two band buffers alternate between the pairs / tiles; the
-// accumulator is double-buffered in TMEM so a tile's epilogue overlaps the next tile's MMAs.
+// Roles (288 threads, one CTA per SM, persistent over tiles): warps 0-7 = two consumer warpgroups (rows 64g..64g+63
+// of a tile, register accumulators, epilogue -> fp32 NCHW planes or bf16 padded NHWC), warp 8 = TMA producer.  Up to
+// four band buffers are in flight, so the next tiles' loads overlap a tile's epilogue.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -36,7 +34,8 @@ namespace {
 using namespace bbtc;
 
 constexpr int BM = 128, BN = 64;
-constexpr int NTHREADS = 192;
+constexpr int NTHREADS = 288;                 // 2 consumer warpgroups + the TMA producer warp
+constexpr int PRODUCER_WARP = 8;
 constexpr int BAND_ROWS = 256;                 // TMA box limit; a band needs 128 + 2*(W+2) + 2 rows
 constexpr int BAND_BYTES = BAND_ROWS * 128;    // 32 KB
 constexpr int W_TILE = 64 * 128;               // one tap's weights: 64 rows (n) x 64 ch
@@ -59,14 +58,12 @@ struct alignas(64) HaloArgs {
                              // row tile*128 + r of the output matrix: one contiguous 16 KB block per tile), border rows 0
   int beta;
   const float* bias;
-  int bo_mode;               // 1: descriptor base offset = (start >> 7) & 7 (PTX ISA), 0: always 0
 };
 
 
 // Shared memory: [npairs x 9 x 8 KB] weights (resident for the whole kernel) | [NB x band_alloc] activation bands |
-// barriers.  The MMA issue loop must stay free of waits: a variant that streamed the second pair's weights through a
-// ring (mbarrier wait + commit per tap inside the tap loop) ran 1.9x slower even with the ring path never taken
-// (554 vs 297 us at 800x42x42, tools/halo_bench.py), so both pairs' weights stay resident and two bands are in flight.
+// barriers.  The MMA issue loop stays free of waits: both pairs' weights are resident rather than streamed through a
+// ring with a wait per tap, and two bands are in flight.
 template <int NB, bool BF16OUT>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_constant__ HaloArgs G) {
   extern __shared__ uint8_t smem_raw[];
@@ -76,30 +73,20 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
   uint64_t* bars = reinterpret_cast<uint64_t*>(bands + (size_t)NB * G.band_alloc);
   const uint32_t wfull = smem_u32(bars);
   const uint32_t bfull0 = smem_u32(bars + 1), bempty0 = smem_u32(bars + 1 + MAXBAND);
-  const uint32_t accf0 = smem_u32(bars + 1 + 2 * MAXBAND), acce0 = accf0 + 16;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 5 + 2 * MAXBAND);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   if (tid == 0) {
     mbar_init(wfull, 1);
     for (int b = 0; b < MAXBAND; ++b) {
       mbar_init(bfull0 + 8 * b, 1);
-      mbar_init(bempty0 + 8 * b, 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(accf0 + 8 * b, 1);
-      mbar_init(acce0 + 8 * b, 4);
+      mbar_init(bempty0 + 8 * b, 2);   // one arrival per consumer warpgroup
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), (uint32_t)(2 * BN));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t band_bytes = (uint32_t)G.band_rows * 128u;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ---------------- TMA producer: activation bands (+ the resident weights once) ----------------
     if (elect_one()) {
       for (int p = 0; p < G.npairs; ++p) {
@@ -120,131 +107,84 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
         }
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer ----------------
-    // One elected thread; everything the 36 instructions of a (tile, pair) need is a 32-bit add away: the descriptors'
-    // constant upper half, the nine tap offsets (in 16-byte units) and the weight tiles' addresses are set up once.
-    // With N = 64 an instruction is only ~34 clocks of tensor work, so every scalar instruction between two issues counts
-    // (the first version rebuilt both 64-bit descriptors per instruction and ran at ~108 clocks per instruction).
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16(BM, BN, false, false);
-      const uint64_t dhi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-      uint32_t tap16[9];
-#pragma unroll
-      for (int t = 0; t < 9; ++t) {
-        const int i = t / 3, j = t - 3 * i;
-        const int dy = G.flip ? 1 - i : i - 1, dx = G.flip ? 1 - j : j - 1;
-        tap16[t] = (uint32_t)((G.Wp + 1 + dy * G.Wp + dx) * 8);
-      }
-      const uint32_t w16 = (smem_u32(wsm) & 0x3FFFF) >> 4, band16_0 = (smem_u32(bands) & 0x3FFFF) >> 4;
-      const uint32_t band16_step = (uint32_t)G.band_alloc >> 4;
-      mbar_wait(wfull, 0);
-      tc_fence_after();
-      int git = 0, lt = 0;
-      for (int tile = blockIdx.x; tile < G.ntiles; tile += gridDim.x, ++lt) {
-        const int buf = lt & 1;
-        if (lt >= 2) {
-          mbar_wait(acce0 + 8 * buf, ((lt >> 1) - 1) & 1);
-          tc_fence_after();
-        }
-        const uint32_t tacc = tmem_base + (uint32_t)(buf * BN);
-        for (int p = 0; p < G.npairs; ++p, ++git) {
-          const int b = git % NB;
-          mbar_wait(bfull0 + 8 * b, (git / NB) & 1);
-          tc_fence_after();
-          const uint32_t band16 = band16_0 + (uint32_t)b * band16_step;
-          const uint32_t wp16 = w16 + (uint32_t)p * (9 * W_TILE >> 4);
-#pragma unroll
-          for (int t = 0; t < 9; ++t) {
-            const uint32_t alo = band16 + tap16[t], blo = wp16 + (uint32_t)t * (W_TILE >> 4);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_bf16(tacc, dhi | (uint64_t)(alo + 2 * k), dhi | (uint64_t)(blo + 2 * k), idesc, (p > 0 || t > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(bempty0 + 8 * b);
-        }
-        umma_commit(accf0 + 8 * buf);
-      }
-    }
-    __syncwarp();
-  } else {
-    // ---------------- epilogue (warps 2..5) ----------------
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const int64_t HW = (int64_t)G.H * G.W;
-    int lt = 0;
-    for (int tile = blockIdx.x; tile < G.ntiles; tile += gridDim.x, ++lt) {
-      const int buf = lt & 1;
-      const int64_t row = (int64_t)tile * BM + r;          // padded-linear pixel index
-      bool ok = row < G.total_rows;
-      int64_t obase = 0;
-      if (ok) {
-        const int img = (int)(row / G.HpWp);
-        const int rem = (int)(row - (int64_t)img * G.HpWp);
-        const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
-        ok = yy >= 1 && yy <= G.H && xx >= 1 && xx <= G.W;
-        obase = (int64_t)img * BN * HW + (int64_t)(yy - 1) * G.W + (xx - 1);
-      }
-      mbar_wait(accf0 + 8 * buf, (lt >> 1) & 1, 60);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN + c * 32), v);
-        if (c == BN / 32 - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(acce0 + 8 * buf);
-        }
-        if (BF16OUT) {
-          // bf16 padded-NHWC output: this thread's pixel row, 32 channels = 64 contiguous bytes; border rows are zeros
-          if (row >= G.total_rows) continue;
-          uint4* q = reinterpret_cast<uint4*>(G.out_bf16 + row * 64 + c * 32);
-#pragma unroll
-          for (int jj = 0; jj < 32; jj += 8) {
-            uint4 o;
-            if (ok) {
-              float f[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) f[e] = __uint_as_float(v[jj + e]) + (G.bias ? G.bias[c * 32 + jj + e] : 0.f);
-              __nv_bfloat162 p0 = __floats2bfloat162_rn(f[0], f[1]), p1 = __floats2bfloat162_rn(f[2], f[3]);
-              __nv_bfloat162 p2 = __floats2bfloat162_rn(f[4], f[5]), p3 = __floats2bfloat162_rn(f[6], f[7]);
-              o.x = *reinterpret_cast<uint32_t*>(&p0); o.y = *reinterpret_cast<uint32_t*>(&p1);
-              o.z = *reinterpret_cast<uint32_t*>(&p2); o.w = *reinterpret_cast<uint32_t*>(&p3);
-            } else {
-              o = make_uint4(0, 0, 0, 0);
-            }
-            q[jj >> 3] = o;
-          }
-          continue;
-        }
-        if (!ok) continue;
-        float* q = G.out + obase + (int64_t)(c * 32) * HW;
-        if (G.bias) {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) v[jj] = __float_as_uint(__uint_as_float(v[jj]) + G.bias[c * 32 + jj]);
-        }
-        if (G.beta) {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) {
-            *q += __uint_as_float(v[jj]);
-            q += HW;
-          }
-        } else {
-#pragma unroll
-          for (int jj = 0; jj < 32; ++jj) {
-            *q = __uint_as_float(v[jj]);
-            q += HW;
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)(2 * BN));
+  // ---------------- consumers (warpgroups 0, 1) ----------------
+  // Everything the 36 wgmma of a (tile, pair) need is a 32-bit add away: the descriptors' constant upper half, the nine
+  // tap offsets (in 16-byte units) and the weight tiles' addresses are set up once.
+  const int wg = tid >> 7, t = tid & 127;
+  const uint64_t dhi = ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | kDescSw128;
+  uint32_t tap16[9];
+#pragma unroll
+  for (int q = 0; q < 9; ++q) {
+    const int i = q / 3, j = q - 3 * i;
+    const int dy = G.flip ? 1 - i : i - 1, dx = G.flip ? 1 - j : j - 1;
+    tap16[q] = (uint32_t)((G.Wp + 1 + dy * G.Wp + dx + wg * 64) * 8);
+  }
+  const uint32_t w16 = (smem_u32(wsm) & 0x3FFFF) >> 4, band16_0 = (smem_u32(bands) & 0x3FFFF) >> 4;
+  const uint32_t band16_step = (uint32_t)G.band_alloc >> 4;
+  const int64_t HW = (int64_t)G.H * G.W;
+  mbar_wait(wfull, 0);
+  float acc[BN / 2];
+  int git = 0;
+  for (int tile = blockIdx.x; tile < G.ntiles; tile += gridDim.x) {
+    for (int p = 0; p < G.npairs; ++p, ++git) {
+      const int b = git % NB;
+      mbar_wait(bfull0 + 8 * b, (git / NB) & 1);
+      const uint32_t band16 = band16_0 + (uint32_t)b * band16_step;
+      const uint32_t wp16 = w16 + (uint32_t)p * (9 * W_TILE >> 4);
+      fence_acc(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int q = 0; q < 9; ++q) {
+        const uint32_t alo = band16 + tap16[q], blo = wp16 + (uint32_t)q * (W_TILE >> 4);
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_n64<0, 0>(acc, dhi | (uint64_t)(alo + 2 * k), dhi | (uint64_t)(blo + 2 * k), (p > 0 || q > 0 || k > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      fence_acc(acc);
+      wgmma_wait<1>();
+      if (p > 0 && t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
+    }
+    wgmma_wait<0>();
+    fence_acc(acc);
+    if (t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
+    // ---------------- epilogue: d[4j + 2h + e] = (row frag_row + 8h, channel 8j + frag_col + e) ----------------
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int64_t row = (int64_t)tile * BM + wg * 64 + frag_row(t) + 8 * h;   // padded-linear pixel index
+      if (row >= G.total_rows) continue;
+      const int img = (int)(row / G.HpWp);
+      const int rem = (int)(row - (int64_t)img * G.HpWp);
+      const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
+      const bool ok = yy >= 1 && yy <= G.H && xx >= 1 && xx <= G.W;
+      if (BF16OUT) {
+        // bf16 padded-NHWC output: this pixel row's 64 channels; border rows are zeros
+        __nv_bfloat162* q = reinterpret_cast<__nv_bfloat162*>(G.out_bf16 + row * 64 + frag_col(t));
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int n = 8 * j + frag_col(t);
+          float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+          if (G.bias) { f0 += G.bias[n]; f1 += G.bias[n + 1]; }
+          q[4 * j] = ok ? __floats2bfloat162_rn(f0, f1) : __floats2bfloat162_rn(0.f, 0.f);
+        }
+        continue;
+      }
+      if (!ok) continue;
+      float* q = G.out + (int64_t)img * BN * HW + (int64_t)(yy - 1) * G.W + (xx - 1);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int n = 8 * j + frag_col(t) + e;
+          float v = acc[4 * j + 2 * h + e];
+          if (G.bias) v += G.bias[n];
+          float* d = q + (int64_t)n * HW;
+          *d = G.beta ? *d + v : v;
+        }
+      }
+    }
   }
 }
 
@@ -252,9 +192,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
 // Weight gradient with the same halo trick:  D[tap][c][o] += sum_pixels X[pixel + d(tap)][c] * G[pixel][o]
 // Both operands are MN-major (rows = pixels = the reduction dimension), X and G in the padded NHWC layout.  Per tile of
 // 128 padded-linear pixels: ONE TMA box of G (128 rows) and ONE band of X (128 + 2(W+2) + 2 rows); the nine taps are
-// nine row offsets into the X band, two taps per M=128 instruction (the MN-major leading-dimension byte offset is the
-// row distance between the two taps).  wgrad_tma_kernel (conv_tma.cu) loads one X box per tap and tile of <= 64 pixels.
-// Accumulators stay in TMEM over all tiles of the CTA (5 x 64 columns); one atomic flush per CTA at the end.
+// nine row offsets into the X band.  Three consumer warpgroups split the taps (warpgroup g owns taps g, g+3, g+6, one
+// wgmma m64n64 per tap and 16-pixel step); wgrad_tma_kernel (conv_tma.cu) loads one X box per tap and tile of <= 64
+// pixels.  Accumulators stay in registers over all tiles of the CTA; each CTA writes them to its own slice of `part` and
+// bb_partials_reduce adds the slices in CTA order (the result does not depend on which CTA finished first).
 // ---------------------------------------------------------------------------------------------------------------
 struct alignas(64) WHaloArgs {
   CUtensorMap x[2], g[2];
@@ -264,38 +205,34 @@ struct alignas(64) WHaloArgs {
   int64_t total_rows;
   int ntiles;
   int stages;
-  float* out;                 // [64 (o)][64 (c)][9] fp32, accumulated with atomics
+  float* part;                // [gridDim.x][O][C][9] fp32 per-CTA partial sums
   int C, O;
 };
 
 constexpr int WH_G_BYTES = 128 * 128;     // 16 KB
 constexpr int WH_STAGE = BAND_BYTES + WH_G_BYTES;
+constexpr int WH_CONSUMERS = 3;
+constexpr int WH_THREADS = WH_CONSUMERS * 128 + 32;
 
-__global__ void __launch_bounds__(NTHREADS, 1) wgrad_halo_kernel(const __grid_constant__ WHaloArgs G) {
+__global__ void __launch_bounds__(WH_THREADS, 1) wgrad_halo_kernel(const __grid_constant__ WHaloArgs G) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + G.stages * WH_STAGE);
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 4), accum = smem_u32(bars + 8);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 4);
+  const int tid = threadIdx.x, warp = tid >> 5;
   if (tid == 0) {
     for (int s = 0; s < G.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, WH_CONSUMERS);
     }
-    mbar_init(accum, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int my_tiles = ((int)blockIdx.x < G.ntiles) ? (G.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   const int total = my_tiles * G.npairs;
   const uint32_t bytes = (uint32_t)G.band_rows * 128u + (uint32_t)WH_G_BYTES;
 
-  if (warp == 0) {
+  if (warp == WH_CONSUMERS * 4) {
     if (elect_one()) {
       for (int p = 0; p < G.npairs; ++p) {
         tma_prefetch_desc(&G.x[p]);
@@ -314,74 +251,96 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad_halo_kernel(const __grid_co
         tma_load_3d(base + BAND_BYTES, &G.g[pair], bar, 0, m0, 0);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16(128, 64, true, true);
-      // descriptor halves set up once (see conv_halo_kernel): per instruction only the 32-bit start addresses change
-      const uint64_t dhi = ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)1 << 46) | ((uint64_t)2 << 61);
-      const uint64_t ghi = dhi | ((uint64_t)(8192 >> 4) << 16);
-      uint64_t xhi[5];
-      uint32_t x16[5];
+    return;
+  }
+  const int wg = tid >> 7, t = tid & 127;
+  // descriptor halves set up once (see conv_halo_kernel): per instruction only the 32-bit start addresses change; one
+  // 64-wide MN block per operand, so the leading byte offset is never used
+  const uint64_t dhi = ((uint64_t)(8192 >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | kDescSw128;
+  uint32_t x16[3];
 #pragma unroll
-      for (int tp = 0; tp < 5; ++tp) {
-        const int t1 = 2 * tp, t2 = (2 * tp + 1 < 9) ? 2 * tp + 1 : 2 * tp;
-        const int d1 = (t1 / 3 - 1) * G.Wp + (t1 % 3 - 1), d2 = (t2 / 3 - 1) * G.Wp + (t2 % 3 - 1);
-        const uint32_t lbo = t2 == t1 ? 128u : (uint32_t)((d2 - d1) * 128);   // (tap 8 alone: the upper half is ignored)
-        xhi[tp] = dhi | ((uint64_t)(lbo >> 4) << 16);
-        x16[tp] = (uint32_t)((G.Wp + 1 + d1) * 8);
-      }
-      for (int it = 0; it < total; ++it) {
-        const int s = it % G.stages;
-        mbar_wait(full0 + 8 * s, (it / G.stages) & 1);
-        tc_fence_after();
-        const uint32_t band16 = (smem_u32(smem + s * WH_STAGE) & 0x3FFFF) >> 4, g16 = band16 + (BAND_BYTES >> 4);
+  for (int q = 0; q < 3; ++q) {
+    const int tap = wg + WH_CONSUMERS * q;
+    x16[q] = (uint32_t)((G.Wp + 1 + (tap / 3 - 1) * G.Wp + (tap % 3 - 1)) * 8);
+  }
+  float acc[3][32];
 #pragma unroll
-        for (int tp = 0; tp < 5; ++tp) {
-          const uint32_t xa = band16 + x16[tp];
+  for (int q = 0; q < 3; ++q)
 #pragma unroll
-          for (int ks = 0; ks < 8; ++ks)
-            umma_bf16(tmem_base + (uint32_t)(tp * 64), xhi[tp] | (uint64_t)(xa + ks * 128), ghi | (uint64_t)(g16 + ks * 128),
-                      idesc, (it > 0 || ks > 0) ? 1u : 0u);
-        }
-        umma_commit(empty0 + 8 * s);
-      }
-      if (total > 0) umma_commit(accum);
+    for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+  for (int it = 0; it < total; ++it) {
+    const int s = it % G.stages;
+    mbar_wait(full0 + 8 * s, (it / G.stages) & 1);
+    const uint32_t band16 = (smem_u32(smem + s * WH_STAGE) & 0x3FFFF) >> 4, g16 = band16 + (BAND_BYTES >> 4);
+#pragma unroll
+    for (int q = 0; q < 3; ++q) fence_acc(acc[q]);
+    wgmma_fence();
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      const uint32_t xa = band16 + x16[q];
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks)
+        wgmma_n64<1, 1>(acc[q], dhi | (uint64_t)(xa + ks * 128), dhi | (uint64_t)(g16 + ks * 128), (it > 0 || ks > 0) ? 1u : 0u);
     }
-    __syncwarp();
-  } else {
-    if (total > 0) {
-      mbar_wait(accum, 0, 200);
-      tc_fence_after();
-      const int quarter = warp & 3;
-      const int L = quarter * 32 + lane;
-      const int half = L >> 6, c = L & 63;
-#pragma unroll 1
-      for (int tp = 0; tp < 5; ++tp) {
-        const int tap = 2 * tp + half;
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(tp * 64 + cc * 32), v);
-          if (tap < 9 && c < G.C) {
+    wgmma_commit();
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int o = cc * 32 + j;
-              if (o < G.O) atomicAdd(G.out + ((int64_t)o * G.C + c) * 9 + tap, __uint_as_float(v[j]));
-            }
-          }
+    for (int q = 0; q < 3; ++q) fence_acc(acc[q]);
+    wgmma_wait<1>();
+    if (it > 0 && t == 0) mbar_arrive(empty0 + 8 * ((it - 1) % G.stages));
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int q = 0; q < 3; ++q) {
+    fence_acc(acc[q]);
+    const int tap = wg + WH_CONSUMERS * q;
+    // d[4j + 2h + e]: row c = frag_row + 8h, column o = 8j + frag_col + e
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int c = frag_row(t) + 8 * h;
+      if (c >= G.C) continue;
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int o = 8 * j + frag_col(t) + e;
+          if (o < G.O) G.part[((int64_t)blockIdx.x * G.O * G.C + (int64_t)o * G.C + c) * 9 + tap] = acc[q][4 * j + 2 * h + e];
         }
-      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
+}
+
+__global__ void __launch_bounds__(256) partials_reduce_kernel(const float* __restrict__ part, int parts, int64_t n,
+                                                              float* __restrict__ out) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    float v = 0.f;
+    for (int b = 0; b < parts; ++b) v += part[(int64_t)b * n + i];
+    out[i] += v;
   }
 }
 
 }  // namespace
+
+int bb_partials_reduce(const float* part, int parts, int64_t n, float* out, cudaStream_t s) {
+  int64_t blocks = (n + 255) / 256;
+  if (blocks > 4 * BB_SM_COUNT) blocks = 4 * BB_SM_COUNT;
+  partials_reduce_kernel<<<(unsigned)blocks, 256, 0, s>>>(part, parts, n, out);
+  bb_launch_tally += 1;
+  BB_LAUNCH_CHECK();
+  return BB_OK;
+}
+
+float* bb_partials_acquire(size_t bytes, cudaStream_t s, bool* owned) {
+  *owned = false;
+  if (float* p = bb_reduce_ws_get(bytes)) return p;
+  void* p = nullptr;
+  if (cudaMallocAsync(&p, bytes, s) != cudaSuccess) return nullptr;
+  *owned = true;
+  return reinterpret_cast<float*>(p);
+}
+
+void bb_partials_release(float* p, bool owned, cudaStream_t s) {
+  if (owned) cudaFreeAsync(p, s);
+}
 
 bool bb_conv_halo_ok(int C, int O, int H, int W) {
   static const bool off = getenv("BB200_NO_HALO") != nullptr;
@@ -403,11 +362,6 @@ int bb_conv_halo_run(int N, int H, int W, int npairs, const void* const* act_pad
   G.out = out; G.beta = beta; G.bias = bias;
   G.out_bf16 = reinterpret_cast<__nv_bfloat16*>(out_bf16_padded);
   if (G.out_bf16 ? beta != 0 : out == nullptr) return BB_ERR_ARG;
-  // measured on B200 (tests/test_conv_halo_gpu.py, GPU call #52): SWIZZLE_128B is a pure function of the shared-memory
-  // address bits, so a descriptor that starts on any 128-byte row reads the TMA-written band correctly with base offset 0
-  // (setting the field to (start >> 7) & 7 gives wrong products); BB200_HALO_BO=1 keeps the other convention testable
-  static const int bo_env = getenv("BB200_HALO_BO") ? atoi(getenv("BB200_HALO_BO")) : 0;
-  G.bo_mode = bo_env;
   G.band_rows = (G.band_rows + 7) & ~7;
   int rc;
   for (int p = 0; p < npairs; ++p) {
@@ -467,7 +421,7 @@ int bb_wgrad_halo_run(int N, int H, int W, int C, int O, int npairs, const void*
   G.total_rows = (int64_t)N * (H + 2) * (W + 2);
   G.ntiles = (int)((G.total_rows + BM - 1) / BM);
   G.stages = 4;
-  G.out = out; G.C = C; G.O = O;
+  G.C = C; G.O = O;
   int rc;
   for (int p = 0; p < npairs; ++p) {
     if ((rc = bb_tma_map_2d(&G.x[p], x_padded[p], G.total_rows, 64, 64, G.band_rows))) return rc;
@@ -478,15 +432,25 @@ int bb_wgrad_halo_run(int N, int H, int W, int C, int O, int npairs, const void*
   if (configured.need())
     BB_CUDA_TRY(cudaFuncSetAttribute(wgrad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const int grid = G.ntiles < BB_SM_COUNT ? G.ntiles : BB_SM_COUNT;
-  wgrad_halo_kernel<<<grid, NTHREADS, smem, s>>>(G);
+  const int64_t n = (int64_t)O * C * 9;
+  bool owned = false;
+  G.part = bb_partials_acquire(sizeof(float) * grid * n, s, &owned);
+  if (G.part == nullptr) return cudaErrorMemoryAllocation;
+  wgrad_halo_kernel<<<grid, WH_THREADS, smem, s>>>(G);
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
-  return BB_OK;
+  rc = bb_partials_reduce(G.part, grid, n, out, s);
+  bb_partials_release(G.part, owned, s);
+  return rc;
 }
 
 extern "C" int bb_wgrad_halo_bf16(int N, int H, int W, int npairs, const void* x0, const void* x1, const void* g0, const void* g1,
                                   float* out, void* stream) {
   const void* xs[2] = {x0, x1};
   const void* gs[2] = {g0, g1};
-  return bb_wgrad_halo_run(N, H, W, 64, 64, npairs, xs, gs, out, (cudaStream_t)stream);
+  const BbReduceWs saved = bb_reduce_ws;   // not a plan pass: no plan workspace (its stream may be elsewhere)
+  bb_reduce_ws = BbReduceWs{nullptr, 0};
+  const int rc = bb_wgrad_halo_run(N, H, W, 64, 64, npairs, xs, gs, out, (cudaStream_t)stream);
+  bb_reduce_ws = saved;
+  return rc;
 }

@@ -13,6 +13,6 @@ int bb_conv_halo_run(int N, int H, int W, int npairs, const void* const* act_pad
 // out_bf16_padded != nullptr: the result is written as bf16 in the padded NHWC layout instead (one contiguous 16 KB
 // block per 128-pixel tile, border rows zero) -- directly the next kernel's TMA operand; `out` / `beta` unused
 // weight gradient over padded operands: out[o][c][tap] += sum_pairs sum_pixels gy[pair][pixel][o] * x[pair][pixel + d(tap)][c]
-// (out: fp32 [O][C][9], accumulated with atomics)
+// (out: fp32 [O][C][9], accumulated: per-CTA partials added in CTA order)
 int bb_wgrad_halo_run(int N, int H, int W, int C, int O, int npairs, const void* const* x_padded, const void* const* gy_padded,
                       float* out, cudaStream_t s);

@@ -1,9 +1,8 @@
 // K6, small-channel convolutions (LeNet-class), second generation of conv_small.cu (which stays as the fallback for
 // geometries these kernels decline).  Exact fp32 on the FMA pipe: the 1e-4 parity bar rules out single-pass TF32 and
 // these layers (<= 16 channels) are FMA-bound, not HBM-bound -- LeNet B=4096 needs 10.3 G multiply-adds per K-loop
-// iteration = 0.28 ms at the 37 TFMA/s fp32 peak against 0.11 ms of HBM time (SURVEY 8d bytes).  The first-generation
-// kernels reached 14 % (wgrad) / 27 % (corr) of the FMA peak (profiles/r01_traffic_ncu.md: issue slots 70 % busy, a
-// shared-memory or global load for every 2.5 ... 5 FMAs, 2x zero-padding work in the data-gradient form).
+// iteration against 0.72 GB of HBM traffic (SURVEY 8d bytes).  The first-generation kernels issue a shared-memory or
+// global load for every 2.5 ... 5 FMAs and do 2x zero-padding work in the data-gradient form.
 //
 //   conv_small_corr2_kernel   out[n,co,y,x] = sum_p sum_{ci,i,j} in_p[n,ci,y-ph+i,x-pw+j] * w_p(co,ci,i,j)  (+bias)
 //       (forward and data-gradient indexing as in conv_small.cu).  A warp owns ONE output row y of IMGS images: lane =
@@ -459,8 +458,8 @@ bool wgrad2_plan(const SmallConvArgs& A, int OB, Wgrad2Geom& G, size_t& smem) {
   G.OPs = (G.OG * OB + 3) & ~3;
   G.tasks = G.OG * C * A.KH;
   if (G.tasks > 256 || G.tasks < 1) return false;
-  // measured (profiles/r02_lenet_small_conv.md): with few tasks per image (LeNet conv1: 15) a block needs ~17 row slices
-  // and its per-image barriers dominate -- the first-generation kernel is faster there (0.32 vs 0.43 ms)
+  // with few tasks per image (LeNet conv1: 15) a block needs ~17 row slices and its per-image barriers dominate -- the
+  // first-generation kernel is faster there
   if (G.tasks < 64 && !getenv("BB200_WGRAD2_ALWAYS")) return false;
   G.ns = 256 / G.tasks;
   if (G.ns > A.HO) G.ns = A.HO;

@@ -11,10 +11,10 @@
 //
 // wgrad: D_tap[c][o] = sum_pixels X[pixel + tap][c] * G[pixel][o] has its reduction over pixels, so both operands are
 // MN-major tiles (rows = pixels = k) -- exactly what the NHWC boxes are.  One CTA walks a strided set of pixel tiles;
-// per tile the TMA brings one G box and one shifted X box per tap; the MMA warp issues M=128 instructions that cover
-// two taps at once (the MN-major leading-dimension byte offset jumps from one tap's tile to the next) into
-// ceil(taps/2) TMEM accumulators of 64 columns; the epilogue adds the CTA's partial sums into the fp32 weight
-// adjoint with atomics.
+// per tile the TMA brings one G box and one shifted X box per tap; three consumer warpgroups split the taps (warpgroup
+// g owns taps g, g+3, g+6) and issue one wgmma m64n64 per tap and 16-pixel step into register accumulators that live
+// over all tiles of the CTA; the epilogue writes the CTA's partial sums to its own slice of `part`, and
+// bb_partials_reduce adds the slices into the fp32 weight adjoint in CTA order.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -31,7 +31,8 @@ namespace {
 
 using namespace bbtc;
 
-constexpr int WG_THREADS = 192;
+constexpr int WG_CONSUMERS = 3;                      // warpgroups; up to 3 taps each
+constexpr int WG_THREADS = WG_CONSUMERS * 128 + 32;    // + the TMA producer warp
 constexpr int WG_MAX_TAPS = 9;
 
 struct alignas(64) WgradArgs {
@@ -42,22 +43,19 @@ struct alignas(64) WgradArgs {
   int tiles_per_img, ntiles;
   int stages;
   int C, O;                 // real channel counts (<= 64)
-  float* out;               // W-shaped [O][C][taps] fp32, accumulated with atomics
+  float* part;              // [gridDim.x][O][C][taps] fp32 per-CTA partial sums
 };
 
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tma_kernel(const __grid_constant__ WgradArgs G) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int tile_bytes = G.RK * 128;
-  const int npairs_tap = (G.taps + 1) / 2;          // M=128 instructions per k-step
-  const int ntile_slots = 2 * npairs_tap + 1;       // X tiles (even count, last may stay zero) + G tile
-  const int stage_bytes = ntile_slots * tile_bytes;
+  const int stage_bytes = (G.taps + 1) * tile_bytes;   // X tile per tap + G tile
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + G.stages * stage_bytes);
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 4), accum = smem_u32(bars + 8);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + 4);
+  const int tid = threadIdx.x, warp = tid >> 5;
 
-  // zero the stage buffers once: rows the TMA never writes (tile tail, the unused odd tap slot) must read as 0
+  // zero the stage buffers once: rows the TMA never writes (tile tail) must read as 0
   {
     uint4* z = reinterpret_cast<uint4*>(smem);
     const int n16 = G.stages * stage_bytes / 16;
@@ -67,21 +65,16 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tma_kernel(const __grid_c
   if (tid == 0) {
     for (int s = 0; s < G.stages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, WG_CONSUMERS);
     }
-    mbar_init(accum, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   const int my_tiles = ((int)blockIdx.x < G.ntiles) ? (G.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   const int total = my_tiles * G.npairs;
 
-  if (warp == 0) {
+  if (warp == WG_CONSUMERS * 4) {
     if (elect_one()) {
       for (int p = 0; p < G.npairs; ++p) {
         tma_prefetch_desc(&G.x[p]);
@@ -97,66 +90,66 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tma_kernel(const __grid_c
         const uint32_t bar = full0 + 8 * s;
         const uint32_t base = smem_u32(smem + s * stage_bytes);
         mbar_expect_tx(bar, bytes);
-        tma_load_4d(base + 2 * npairs_tap * tile_bytes, &G.g[pair], bar, 0, 0, h0, img);
+        tma_load_4d(base + G.taps * tile_bytes, &G.g[pair], bar, 0, 0, h0, img);
         for (int t = 0; t < G.taps; ++t) {
           const int i = t / G.KW, j = t - i * G.KW;
           tma_load_4d(base + t * tile_bytes, &G.x[pair], bar, 0, j - G.pw, h0 + i - G.ph, img);
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      const uint32_t idesc = idesc_bf16(128, 64, true, true);
-      const int ksteps = G.RK / 16;
-      for (int it = 0; it < total; ++it) {
-        const int s = it % G.stages;
-        mbar_wait(full0 + 8 * s, (it / G.stages) & 1);
-        tc_fence_after();
-        const uint32_t base = smem_u32(smem + s * stage_bytes);
-        const uint32_t g_addr = base + 2 * npairs_tap * tile_bytes;
-        for (int tp = 0; tp < npairs_tap; ++tp) {
-          const uint32_t x_addr = base + 2 * tp * tile_bytes;
-          for (int ks = 0; ks < ksteps; ++ks) {
-            const uint64_t da = desc_mn(x_addr + ks * 2048, (uint32_t)tile_bytes);
-            const uint64_t db = desc_mn(g_addr + ks * 2048, 8192);
-            umma_bf16(tmem_base + (uint32_t)(tp * 64), da, db, idesc, (it > 0 || ks > 0) ? 1u : 0u);
-          }
-        }
-        umma_commit(empty0 + 8 * s);
-      }
-      if (total > 0) umma_commit(accum);
-    }
-    __syncwarp();
   } else {
-    if (total > 0) {
-      mbar_wait(accum, 0, 200);
-      tc_fence_after();
-      const int quarter = warp & 3;
-      const int L = quarter * 32 + lane;
-      const int half = L >> 6, c = L & 63;
-#pragma unroll 1
-      for (int tp = 0; tp < npairs_tap; ++tp) {
-        const int tap = 2 * tp + half;
-#pragma unroll 1
-        for (int cc = 0; cc < 2; ++cc) {
-          uint32_t v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(tp * 64 + cc * 32), v);
-          if (tap < G.taps && c < G.C) {
+    const int wg = tid >> 7, t = tid & 127;
+    float acc[3][32];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int o = cc * 32 + j;
-              if (o < G.O) atomicAdd(G.out + ((int64_t)o * G.C + c) * G.taps + tap, __uint_as_float(v[j]));
-            }
-          }
+    for (int q = 0; q < 3; ++q)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[q][i] = 0.f;
+    const int ksteps = G.RK / 16;
+    for (int it = 0; it < total; ++it) {
+      const int s = it % G.stages;
+      mbar_wait(full0 + 8 * s, (it / G.stages) & 1);
+      const uint32_t base = smem_u32(smem + s * stage_bytes);
+      const uint32_t g_addr = base + G.taps * tile_bytes;
+#pragma unroll
+      for (int q = 0; q < 3; ++q) fence_acc(acc[q]);
+      wgmma_fence();
+#pragma unroll
+      for (int q = 0; q < 3; ++q) {
+        const int tap = wg + WG_CONSUMERS * q;
+        if (tap < G.taps) {
+          const uint32_t x_addr = base + tap * tile_bytes;
+          for (int ks = 0; ks < ksteps; ++ks)
+            wgmma_n64<1, 1>(acc[q], desc_mn(x_addr + ks * 2048, 8192), desc_mn(g_addr + ks * 2048, 8192),
+                            (it > 0 || ks > 0) ? 1u : 0u);
         }
       }
+      wgmma_commit();
+#pragma unroll
+      for (int q = 0; q < 3; ++q) fence_acc(acc[q]);
+      wgmma_wait<1>();
+      if (it > 0 && t == 0) mbar_arrive(empty0 + 8 * ((it - 1) % G.stages));
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      fence_acc(acc[q]);
+      const int tap = wg + WG_CONSUMERS * q;
+      if (tap >= G.taps) continue;
+      // d[4j + 2h + e]: row c = frag_row + 8h, column o = 8j + frag_col + e
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int c = frag_row(t) + 8 * h;
+        if (c >= G.C) continue;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int o = 8 * j + frag_col(t) + e;
+            if (o < G.O)
+              G.part[((int64_t)blockIdx.x * G.O * G.C + (int64_t)o * G.C + c) * G.taps + tap] = acc[q][4 * j + 2 * h + e];
+          }
+      }
+    }
   }
 }
 
@@ -214,9 +207,7 @@ int launch_wgrad(const Geo& g, int npairs, const void* const* xs, const void* co
   A.Hb = Hb; A.rows = g.WO * Hb; A.RK = round_up(A.rows, 16);
   A.tiles_per_img = (g.HO + Hb - 1) / Hb; A.ntiles = g.N * A.tiles_per_img;
   A.C = g.C; A.O = g.O;
-  A.out = out;
-  const int slots = 2 * ((taps + 1) / 2) + 1;
-  const size_t stage = (size_t)slots * A.RK * 128;
+  const size_t stage = (size_t)(taps + 1) * A.RK * 128;
   int stages = (int)((220 * 1024 - 2048) / stage);
   if (stages > 4) stages = 4;
   if (stages < 2) return BB_DECLINED;
@@ -227,10 +218,16 @@ int launch_wgrad(const Geo& g, int npairs, const void* const* xs, const void* co
     BB_CUDA_TRY(cudaFuncSetAttribute(wgrad_tma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024));
   }
   const int grid = A.ntiles < BB_SM_COUNT ? A.ntiles : BB_SM_COUNT;
+  const int64_t n = (int64_t)g.O * g.C * taps;
+  bool owned = false;
+  A.part = bb_partials_acquire(sizeof(float) * grid * n, s, &owned);
+  if (A.part == nullptr) return cudaErrorMemoryAllocation;
   wgrad_tma_kernel<<<grid, WG_THREADS, smem, s>>>(A);
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
-  return BB_OK;
+  rc = bb_partials_reduce(A.part, grid, n, out, s);
+  bb_partials_release(A.part, owned, s);
+  return rc;
 }
 
 // ---- first-layer convolutions (few input channels, input is data: no tangent, no input gradient) -------------------

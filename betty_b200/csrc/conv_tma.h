@@ -26,6 +26,6 @@ int bb_conv_tma_corr(const BbConvGeo& g, int npairs, const void* const* src_nhwc
                      int ncols, int GH, int GW, int flip, float* out, int beta, const float* bias, cudaStream_t s,
                      bool padded = false);   // padded: the operands are [N][SH+2][SW+2][64] with a zero border
 // weight gradient: out[o][c][tap] += sum_pairs sum_pixels gy[pair][pixel][o] * x[pair][pixel + disp(tap)][c]
-// x: bf16 NHWC [N][H][W][64], gy: bf16 NHWC [N][HO][WO][64]; out accumulates (fp32 atomics)
+// x: bf16 NHWC [N][H][W][64], gy: bf16 NHWC [N][HO][WO][64]; out accumulates (per-CTA partials added in CTA order)
 int bb_conv_tma_wgrad(const BbConvGeo& g, int npairs, const void* const* x_nhwc, const void* const* gy_nhwc, float* out,
                       cudaStream_t s, bool padded = false);

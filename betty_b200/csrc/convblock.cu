@@ -249,7 +249,7 @@ __device__ __forceinline__ void load_x_tile(const CbArgs& A, int n, int hp0, flo
 // Bulk copy of a contiguous global range into shared memory with cp.async (no register staging: every thread has
 // several independent 16-byte requests in flight, so the pooled arrays of a whole tile stream in at DRAM latency
 // once instead of once per window -- the first version of these kernels ran at 10 % of DRAM throughput on exactly
-// that dependency, profiles/r02_convblock_v0_ncu.md).  Falls back to plain loads for unaligned ranges.
+// that dependency).  Falls back to plain loads for unaligned ranges.
 __device__ __forceinline__ void tile_copy_async(void* dst_smem, const void* src, int nbytes) {
   const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst_smem);
   const uintptr_t a = reinterpret_cast<uintptr_t>(src);
@@ -502,7 +502,7 @@ __global__ void __launch_bounds__(NT, 4) cb_tf_kernel(const CbArgs A) {
     __syncthreads();
     if (och) {
       // strength-reduced indices: everything below advances by additions (the first version spent ~50 integer
-      // multiply-adds per window on address arithmetic, profiles/r02_convblock_v1_ncu.md)
+      // multiply-adds per window on address arithmetic)
       int wr = 0, wc = wg;
       while (wc >= WPc) { wc -= WPc; ++wr; }
       int rowbase = 2 * wr * pitch + 2 * wc;                    // xs offset of the window's top-left candidate pixel
@@ -1085,26 +1085,31 @@ __global__ void __launch_bounds__(256, 2) cb_reduce_mma_kernel(const CbArgs A, i
     }
     __syncwarp();
   }
-  // per-CTA partial row: taps k < CKK -> GW columns, k == CKK -> s0
+  // per-CTA partial row: taps k < CKK -> GW columns, k == CKK -> s0.  The lanes of a warp own distinct entries, so the
+  // warps add in turn (warp order, not arrival order: the partial is the same every run)
+  for (int w = 0; w < 8; ++w) {
+    if (warp == w) {
 #pragma unroll
-  for (int mk = 0; mk < 2; ++mk)
+      for (int mk = 0; mk < 2; ++mk)
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
+        for (int j = 0; j < 8; ++j)
 #pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const int k = mk * 16 + gq + (r >> 1) * 8, o = j * 8 + 2 * t + (r & 1);
-        if (k < CKK)
-          atomicAdd(&red[o][k], gw[mk][j][r]);
-        else if (k == CKK)
-          atomicAdd(&red[o][KP + 0], gw[mk][j][r]);
+          for (int r = 0; r < 4; ++r) {
+            const int k = mk * 16 + gq + (r >> 1) * 8, o = j * 8 + 2 * t + (r & 1);
+            if (k < CKK)
+              red[o][k] += gw[mk][j][r];
+            else if (k == CKK)
+              red[o][KP + 0] += gw[mk][j][r];
+          }
+      red[2 * lane][KP + 1] += s1a;
+      red[2 * lane + 1][KP + 1] += s1b;
+      if (!BASE) {
+        red[2 * lane][KP + 2] += s2a;
+        red[2 * lane + 1][KP + 2] += s2b;
       }
-  atomicAdd(&red[2 * lane][KP + 1], s1a);
-  atomicAdd(&red[2 * lane + 1][KP + 1], s1b);
-  if (!BASE) {
-    atomicAdd(&red[2 * lane][KP + 2], s2a);
-    atomicAdd(&red[2 * lane + 1][KP + 2], s2b);
+    }
+    __syncthreads();
   }
-  __syncthreads();
   for (int i = tid; i < 64 * (KP + NSUM); i += 256) A.w.part[(size_t)blockIdx.x * 64 * (KP + NSUM) + i] = (&red[0][0])[i];
 }
 

@@ -29,7 +29,7 @@ struct Mat {  // a (possibly transposed) strided matrix view
 
 inline Mat T(const Mat& m) { return Mat{m.p, m.dt, m.cs, m.rs, m.bs}; }
 
-// does {m*rs + n*cs (+ b*bs)} cover exactly [0, M*N*batch)?  (needed before a memset + atomic split-K)
+// does {m*rs + n*cs (+ b*bs)} cover exactly [0, M*N*batch)?  (needed before the memset + atomic split-K of the tensor-core kernels)
 inline bool dense_block(int64_t M, int64_t N, int64_t batch, int64_t rs, int64_t cs, int64_t bs) {
   bool ok;
   if (M == 1) ok = (cs == 1 || N == 1);
@@ -58,13 +58,13 @@ int vec_mode(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
 
 template <int BM, int BN, int TM, int TN>
 int launch_vec(int mode, const bb::VecOperands& op, const StridedStore& sc, int64_t M, int64_t N, int64_t K, int npairs,
-               int ksplit, dim3 grid, cudaStream_t s) {
+               int ksplit, dim3 grid, float* part, cudaStream_t s) {
   constexpr int T = (BM / TM) * (BN / TN);
   switch (mode & 3) {
-    case 0: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, false, false, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit); break;
-    case 1: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, true, false, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit); break;
-    case 2: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, false, true, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit); break;
-    default: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, true, true, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit);
+    case 0: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, false, false, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit, part); break;
+    case 1: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, true, false, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit, part); break;
+    case 2: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, false, true, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit, part); break;
+    default: bb::tile_gemm_vec_kernel<BM, BN, TM, TN, true, true, StridedStore><<<grid, T, 0, s>>>(op, sc, M, N, K, npairs, ksplit, part);
   }
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
@@ -78,7 +78,7 @@ int run_gemm(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
   if (M <= 0 || N <= 0 || batch <= 0) return BB_OK;
   static const bool no_tma = getenv("BB200_NO_TMA") != nullptr;
   if (tensor_cores && npairs > 0 && batch > 1 && !no_tma) {
-    // batched products (attention): TMA-fed tcgen05 kernel, one grid.z slice per batch
+    // batched products (attention): TMA-fed wgmma kernel, one grid.z slice per batch
     TmaView a[2], b[2];
     for (int p = 0; p < npairs; ++p) {
       a[p] = TmaView{L[p].p, L[p].dt, L[p].rs, L[p].cs, L[p].bs};
@@ -88,7 +88,7 @@ int run_gemm(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
     if (rc != BB_DECLINED) return rc;
   }
   if (tensor_cores && npairs > 0 && bb_gemm_tc_eligible(M, N, K, batch)) {
-    // bf16-autocast configuration: tcgen05 path (operands rounded to bf16, fp32 accumulation in TMEM).
+    // bf16-autocast configuration: wgmma path (operands rounded to bf16, fp32 accumulation in registers).
     // Preferred: operands packed to TMA-addressable bf16 and fed by the TMA unit (gemm_tma.cu); the software-staged
     // kernel takes what that launcher declines (no scratch, odd shapes).
     if (!no_tma) {
@@ -124,8 +124,8 @@ int run_gemm(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
   const bool small_m = M <= 16, small_n = N <= 16 && !small_m;
   // 64x64 tiles unless that leaves most SMs idle: then 32x32 tiles (4x the CTAs)
   const int64_t tiles64 = ((M + 63) / 64) * ((N + 63) / 64) * batch;
-  // measured on LeNet B=4096 (profiles/r02_lenet_small_conv.md): 128 tiles of 64x64 (4x4 per thread) beat 512 tiles of
-  // 32x32 (2x2 per thread, one shared-memory load per FMA) -- only below ~64 big tiles do the small ones pay
+  // 64x64 tiles (4x4 per thread) do four times the FMAs per shared-memory load of 32x32 tiles (2x2 per thread) -- only
+  // below ~64 big tiles do the small ones pay
   static const int mid_below = getenv("BB200_GEMM_MID") ? atoi(getenv("BB200_GEMM_MID")) : 64;
   const bool mid = !small_m && !small_n && tiles64 < mid_below;
   const int BM = small_m ? 16 : (mid ? 32 : 64), BN = small_n ? 16 : (mid ? 32 : 64);
@@ -138,10 +138,9 @@ int run_gemm(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
     if (ksplit > 64) ksplit = 64;
     if (ksplit < 1) ksplit = 1;
   }
-  if (ksplit > 1 && !beta) {
-    BB_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * M * N * batch, s));
-    bb_launch_tally += 1;
-  }
+  // split-K partials go to the plan's reduction workspace and are summed in split order (splitk_reduce_kernel)
+  ksplit = bb_reduce_ws_splits(ksplit, sizeof(float) * M * N * batch);
+  float* part = ksplit > 1 ? bb_reduce_ws.base : nullptr;
   dim3 grid((unsigned)((N + BN - 1) / BN), (unsigned)((M + BM - 1) / BM), (unsigned)(batch * ksplit));
   const int vmode = (small_m || small_n || getenv("BB200_NO_VEC_GEMM")) ? 0 : vec_mode(M, N, K, batch, npairs, L, R);
   if (vmode) {
@@ -151,26 +150,28 @@ int run_gemm(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
       op.b[p] = reinterpret_cast<const float*>(R[p].p);
     }
     op.ars = L[0].rs; op.acs = L[0].cs; op.brs = R[0].rs; op.bcs = R[0].cs;
-    return mid ? launch_vec<32, 32, 2, 2>(vmode, op, sc, M, N, K, npairs, ksplit, grid, s)
-               : launch_vec<64, 64, 4, 4>(vmode, op, sc, M, N, K, npairs, ksplit, grid, s);
+    const int rc = mid ? launch_vec<32, 32, 2, 2>(vmode, op, sc, M, N, K, npairs, ksplit, grid, part, s)
+                       : launch_vec<64, 64, 4, 4>(vmode, op, sc, M, N, K, npairs, ksplit, grid, part, s);
+    return rc ? rc : bb::splitk_reduce(sc, part, M, N, batch, ksplit, s);
   }
   if (small_m)
-    bb::tile_gemm_kernel<16, 64, 16, 1, 4, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit);
+    bb::tile_gemm_kernel<16, 64, 16, 1, 4, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit, part);
   else if (small_n)
-    bb::tile_gemm_kernel<64, 16, 16, 4, 1, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit);
+    bb::tile_gemm_kernel<64, 16, 16, 4, 1, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit, part);
   else if (mid)
-    bb::tile_gemm_kernel<32, 32, 16, 2, 2, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit);
+    bb::tile_gemm_kernel<32, 32, 16, 2, 2, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit, part);
   else
-    bb::tile_gemm_kernel<64, 64, 16, 4, 4, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit);
+    bb::tile_gemm_kernel<64, 64, 16, 4, 4, StridedLoad, StridedLoad, StridedStore><<<grid, 256, 0, s>>>(la, lb, sc, M, N, K, npairs, ksplit, part);
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
-  return BB_OK;
+  return bb::splitk_reduce(sc, part, M, N, batch, ksplit, s);
 }
 
-// out[n] += sum_{b,m} g[b*bs + m*rs + n*cs]   (out must hold the value to accumulate onto)
+// out[n] += sum_{b,m} g[b*bs + m*rs + n*cs]   (out must hold the value to accumulate onto).  With more than one block
+// row (gridDim.y > 1) every block writes its partial to part[blockIdx.y][n] and colsum_finish_kernel adds them in order.
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ g, float* out, int64_t rows_per_b,
                                                      int64_t batch, int64_t N, int64_t rs, int64_t cs, int64_t bs,
-                                                     int64_t out_stride) {
+                                                     int64_t out_stride, float* __restrict__ part) {
   __shared__ float sm[8][33];
   const int64_t n = (int64_t)blockIdx.x * 32 + threadIdx.x;
   const int64_t total = rows_per_b * batch;
@@ -187,8 +188,18 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ g
     float t = 0.f;
 #pragma unroll
     for (int i = 0; i < 8; ++i) t += sm[i][threadIdx.x];
-    atomicAdd(out + n * out_stride, t);
+    if (part != nullptr) part[(int64_t)blockIdx.y * N + n] = t;
+    else out[n * out_stride] += t;
   }
+}
+
+__global__ void __launch_bounds__(256) colsum_finish_kernel(const float* __restrict__ part, int parts, float* out, int64_t N,
+                                                            int64_t out_stride) {
+  const int64_t n = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (n >= N) return;
+  float t = 0.f;
+  for (int i = 0; i < parts; ++i) t += part[(int64_t)i * N + n];
+  out[n * out_stride] += t;
 }
 
 int run_colsum(const float* g, float* out, int64_t M, int64_t batch, int64_t N, int64_t rs, int64_t cs, int64_t bs,
@@ -202,10 +213,17 @@ int run_colsum(const float* g, float* out, int64_t M, int64_t batch, int64_t N, 
   int gy = (int)((rows + 63) / 64);
   if (gy < 1) gy = 1;
   if (gy > 64) gy = 64;
+  gy = bb_reduce_ws_splits(gy, sizeof(float) * N);
+  float* part = gy > 1 ? bb_reduce_ws.base : nullptr;
   dim3 grid((unsigned)((N + 31) / 32), (unsigned)gy);
-  colsum_kernel<<<grid, dim3(32, 8), 0, s>>>(g, out, M, batch, N, rs, cs, bs, out_stride);
+  colsum_kernel<<<grid, dim3(32, 8), 0, s>>>(g, out, M, batch, N, rs, cs, bs, out_stride, part);
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
+  if (part != nullptr) {
+    colsum_finish_kernel<<<(unsigned)((N + 255) / 256), 256, 0, s>>>(part, gy, out, N, out_stride);
+    bb_launch_tally += 1;
+    BB_LAUNCH_CHECK();
+  }
   return BB_OK;
 }
 

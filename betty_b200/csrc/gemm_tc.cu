@@ -1,21 +1,19 @@
-// K5 tensor-core path: dual-product GEMM on the 5th-generation tensor cores (tcgen05.mma, kind::f16 with
-// bf16 operands, fp32 accumulation in TMEM) for the bf16-autocast configurations.
+// K5 tensor-core path: dual-product GEMM on the Hopper tensor cores (wgmma.mma_async with bf16 operands from
+// shared memory, fp32 accumulation in registers) for the bf16-autocast configurations.
 //
 //   D[m][n] (beta/atomic)= sum over up to two operand pairs p of  sum_k A_p[m][k] * B_p[k][n]   (+ bias[n])
 //
-// Operand staging is done by the four producer warps rather than by TMA because the second-order
-// operands are heterogeneous: base activations / weights are bf16 (autocast), tangents and adjoints are
-// fp32 slices of arenas, and half of them are consumed through transposed views.  The producers read
-// global memory with whatever strides the operand has, convert to bf16 and write the canonical K-major
-// SWIZZLE_128B layout the UMMA shared-memory descriptors expect (row pitch 128 B, 16-byte chunk index
-// XOR (row % 8), 8-row groups 1024 B apart), then publish the stage through an mbarrier after a
-// generic->async proxy fence.  One elected thread of the MMA warp issues 4 x tcgen05.mma (M=128, N=128,
-// K=16) per 64-wide k-block into a 128-column TMEM accumulator; tcgen05.commit releases the stage.  After
-// the last k-block the producer warps turn into the epilogue: tcgen05.ld (32 lanes x 32 columns per warp)
-// -> registers -> strided global store with beta / atomic split-K / bias handling.
+// Operand staging is done by the threads themselves rather than by TMA because the second-order operands are
+// heterogeneous: base activations / weights are bf16 (autocast), tangents and adjoints are fp32 slices of arenas,
+// and half of them are consumed through transposed views.  The threads read global memory with whatever strides
+// the operand has, convert to bf16 and write the canonical K-major SWIZZLE_128B layout the wgmma shared-memory
+// descriptors expect (row pitch 128 B, 16-byte chunk index XOR (row % 8), 8-row groups 1024 B apart), then publish
+// the stage with a generic->async proxy fence and a CTA barrier.  Each of the two warpgroups then issues
+// 4 x wgmma m64nBNk16 per 64-wide k-block for its 64 rows of the 128-row tile; the MMAs of k-block i run while
+// k-block i+1 is staged (3-stage ring, wait_group 1).  The epilogue stores the register accumulators with beta /
+// atomic split-K / bias handling.
 //
-// Roles (288 threads): warps 0-7 producers + epilogue (warp w reads TMEM lanes 32*(w%4).. and the (w/4)-th
-// half of the columns), warp 8 MMA issue + TMEM alloc/dealloc.  3-stage ring, 24-32 KB per stage.
+// 256 threads = 2 warpgroups, 24-32 KB per stage.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 
@@ -23,86 +21,16 @@
 #include "bb_common.cuh"
 #include "gemm_tc.h"
 #include "plan.h"
+#include "tc_ptx.cuh"
 
 namespace {
 
 constexpr int BM = 128, BK = 64, STAGES = 3;   // BN = 64 or 128 (template)
-constexpr int NPROD = 256;                   // producer / epilogue threads (8 warps)
-constexpr int NTHREADS = NPROD + 32;
+constexpr int NPROD = 256;                   // staging threads (2 warpgroups)
+constexpr int NTHREADS = NPROD;
 constexpr int TILE_BYTES = BM * BK * 2;      // 16 KB per operand per stage
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
-  uint32_t ok;
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-      "selp.u32 %0, 1, 0, p;\n"
-      "}\n"
-      : "=r"(ok)
-      : "r"(bar), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-// Poll with back-off: a warp spinning on try_wait competes for issue slots with the producer warp that
-// shares its scheduler (ncu: 1.8 M TRYWAIT executions per launch before this was added).
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, unsigned sleep_ns = 40) {
-  while (!mbar_try(bar, parity)) __nanosleep(sleep_ns);
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, version 1):
-// start address >> 4 | LBO(=1, unused for swizzled K-major) << 16 | SBO (1024 B >> 4) << 32 | version 1 << 46 |
-// layout type SWIZZLE_128B (2) << 61
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// MN-major SWIZZLE_128B descriptor (operand stored with the M/N index contiguous): canonical layout
-// ((8,8,m),(8,k)) : ((1,8,LBO),(64,SBO)) in bf16 elements -- an atom is 8 k-rows x 64 mn (1024 B), atoms of one
-// 64-wide mn block are consecutive along k (SBO = 1024 B), the next mn block starts LBO bytes later.
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) @4, a/b_format BF16 (1) @7/@10,
-// a/b major K (0), n_dim = N>>3 @17, m_dim = M>>4 @24 -- see Cfg<BN>::kIdesc
+using namespace bbtc;
 
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
@@ -451,12 +379,9 @@ constexpr int kMaxLutK = 2048;   // 2 tables x 8 B x 2048 = 32 KB
 
 template <int BN_>
 struct Cfg {
-  static constexpr int kBN = BN_;
   static constexpr int kBTile = BN_ * BK * 2;
   static constexpr int kStage = TILE_BYTES + kBTile;
-  static constexpr size_t kSmem = (size_t)STAGES * kStage + 1024 + 128;
-  static constexpr uint32_t kIdesc =
-      (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN_ >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+  static constexpr size_t kSmem = (size_t)STAGES * kStage + 1024;
 };
 
 template <int BN_, int MINB>
@@ -465,13 +390,10 @@ __global__ void __launch_bounds__(NTHREADS, MINB) gemm_tc_kernel(const __grid_co
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B atoms must start on a 1024-byte boundary of the *shared* address space
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::kStage);  // full[3], empty[3], accum, tmem slot
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + STAGES), accum = smem_u32(bars + 2 * STAGES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
-  int2* lut_a = reinterpret_cast<int2*>(reinterpret_cast<uint8_t*>(bars) + 128);
+  int2* lut_a = reinterpret_cast<int2*>(smem + STAGES * C::kStage);
   int2* lut_b = lut_a + G.lut_k;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
   const int64_t m0 = (int64_t)blockIdx.y * BM, n0 = (int64_t)blockIdx.x * BN_;
   const int split = blockIdx.z;
   // k range of this split, in whole k-blocks
@@ -485,119 +407,70 @@ __global__ void __launch_bounds__(NTHREADS, MINB) gemm_tc_kernel(const __grid_co
 
   if (G.a[0].mode == TC_PIXROW || G.a[0].mode == TC_WDGRAD) build_lut(lut_a, G.a[0], G.lut_k, threadIdx.x);
   if (G.b[0].mode == TC_PIXROW || G.b[0].mode == TC_WDGRAD) build_lut(lut_b, G.b[0], G.lut_k, threadIdx.x);
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full0 + 8 * s, NPROD);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    mbar_init(accum, 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == NPROD / 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"((uint32_t)BN_));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < NPROD / 32) {
-    // ---------------- producers ----------------
-    for (int it = 0; it < total_kb; ++it) {
-      const int s = it % STAGES;
-      if (it >= STAGES) mbar_wait(empty0 + 8 * s, ((it / STAGES) - 1) & 1);
-      const int pair = it / nkb;
-      const int64_t k0 = (kb_beg + (it % nkb)) * BK;
-      const int64_t kend = (kb_end * BK < G.K) ? kb_end * BK : G.K;
-      uint8_t* st = smem + s * C::kStage;
-      stage_tile<BM>(st, G.a[pair], m0, G.M, k0, kend, tid, lut_a);
-      stage_tile<BN_>(st + TILE_BYTES, G.b[pair], n0, G.N, k0, kend, tid, lut_b);
-      fence_proxy_async();
-      mbar_arrive(full0 + 8 * s);
+  float acc[BN_ / 2];
+#pragma unroll
+  for (int i = 0; i < BN_ / 2; ++i) acc[i] = 0.f;
+  // Stage s is rewritten at iteration it + 3.  Every warpgroup passed the barrier of iteration it + 2 only after its
+  // wait_group<1> of iteration it + 1, which retires the MMAs of iteration it: the ring needs no other barrier.
+  for (int it = 0; it < total_kb; ++it) {
+    const int s = it % STAGES;
+    const int pair = it / nkb;
+    const int64_t k0 = (kb_beg + (it % nkb)) * BK;
+    const int64_t kend = (kb_end * BK < G.K) ? kb_end * BK : G.K;
+    uint8_t* st = smem + s * C::kStage;
+    stage_tile<BM>(st, G.a[pair], m0, G.M, k0, kend, tid, lut_a);
+    stage_tile<BN_>(st + TILE_BYTES, G.b[pair], n0, G.N, k0, kend, tid, lut_b);
+    fence_proxy_async();
+    __syncthreads();
+    const bool a_mn = G.a[pair].mn_major != 0, b_mn = G.b[pair].mn_major != 0;
+    // this warpgroup's 64 rows: +8 KB in both layouts (64 K-major rows, or the second 64-wide MN block)
+    const uint32_t a_addr = smem_u32(st) + (uint32_t)wg * 8192u, b_addr = smem_u32(st) + TILE_BYTES;
+    fence_acc(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      // K-major tiles advance 32 B per 16-wide k-step inside the 128-byte rows; MN-major tiles advance two
+      // 1024-byte k-atoms
+      const uint64_t da = a_mn ? desc_mn(a_addr + k * 2048, (BK / 8) * 1024) : desc_k(a_addr + k * 32);
+      const uint64_t db = b_mn ? desc_mn(b_addr + k * 2048, (BK / 8) * 1024) : desc_k(b_addr + k * 32);
+      wgmma_bf16<BN_>(acc, da, db, (it > 0 || k > 0) ? 1u : 0u, a_mn, b_mn);
     }
-    // ---------------- epilogue ----------------
-    if (total_kb > 0) {
-      mbar_wait(accum, 0, 200);
-      tc_fence_after();
-    }
-    // warp w reads TMEM lanes 32*(w%4).. (hardware restriction) and the (w/4)-th half of the columns
-    const int quarter = warp & 3, chalf = warp >> 2;
-    const int64_t row = m0 + quarter * 32 + lane;
-    int64_t row_base = 0;
+    wgmma_commit();
+    fence_acc(acc);
+    wgmma_wait<1>();
+  }
+  wgmma_wait<0>();
+  fence_acc(acc);
+
+  // ---------------- epilogue: d[4j + 2h + e] = (row frag_row + 8h, column 8j + frag_col + e) ----------------
+  const int64_t col_stride = G.omode == 1 ? (int64_t)G.OHW : G.ocs;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int64_t row = m0 + wg * 64 + frag_row(t) + 8 * h;
+    if (row >= G.M) continue;
+    int64_t row_base;
     if (G.omode == 1) {
-      const int64_t r = row < G.M ? row : 0;
-      const int64_t img = r / G.OHW, q = r - img * G.OHW;
+      const int64_t img = row / G.OHW, q = row - img * G.OHW;
       row_base = img * G.OCH * G.OHW + q;
     } else {
       row_base = row * G.ors;
     }
-    const int64_t col_stride = G.omode == 1 ? (int64_t)G.OHW : G.ocs;
-#pragma unroll 1
-    for (int c = chalf * (BN_ / 64); c < (chalf + 1) * (BN_ / 64); ++c) {
-      uint32_t r[32];
-      if (total_kb > 0) {
-        const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(c * 32);
-        asm volatile(
-            "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-            "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-            "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-            : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-              "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-              "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-              "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-            : "r"(taddr));
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      } else {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = 0u;
-      }
-      if (row < G.M) {
+    for (int j = 0; j < BN_ / 8; ++j) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int64_t col = n0 + c * 32 + j;
-          if (col < G.N) {
-            float v = __uint_as_float(r[j]);
-            if (G.bias != nullptr && split == 0) v += G.bias[col * G.bias_stride];
-            float* dst = G.out + row_base + col * col_stride;
-            if (G.ksplit > 1) atomicAdd(dst, v);
-            else *dst = G.beta ? *dst + v : v;
-          }
+      for (int e = 0; e < 2; ++e) {
+        const int64_t col = n0 + 8 * j + frag_col(t) + e;
+        if (col < G.N) {
+          float v = acc[4 * j + 2 * h + e];
+          if (G.bias != nullptr && split == 0) v += G.bias[col * G.bias_stride];
+          float* dst = G.out + row_base + col * col_stride;
+          if (G.ksplit > 1) atomicAdd(dst, v);
+          else *dst = G.beta ? *dst + v : v;
         }
       }
     }
-    tc_fence_before();
-  } else {
-    // ---------------- MMA issuer (warp 4, one elected lane) ----------------
-    if (lane == 0) {
-      for (int it = 0; it < total_kb; ++it) {
-        const int s = it % STAGES;
-        const int pair = it / nkb;
-        const bool a_mn = G.a[pair].mn_major != 0, b_mn = G.b[pair].mn_major != 0;
-        const uint32_t idesc = C::kIdesc | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u);
-        mbar_wait(full0 + 8 * s, (it / STAGES) & 1);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * C::kStage), b_addr = a_addr + TILE_BYTES;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          // K-major tiles advance 32 B per 16-wide k-step inside the 128-byte rows; MN-major tiles advance two
-          // 1024-byte k-atoms
-          const uint64_t da = a_mn ? make_desc_mn(a_addr + k * 2048, (BK / 8) * 1024) : make_desc(a_addr + k * 32);
-          const uint64_t db = b_mn ? make_desc_mn(b_addr + k * 2048, (BK / 8) * 1024) : make_desc(b_addr + k * 32);
-          umma_bf16(tmem_base, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(empty0 + 8 * s);   // stage free once these MMAs have read it
-      }
-      if (total_kb > 0) umma_commit(accum);
-    }
-    __syncwarp();
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == NPROD / 32) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)BN_));
   }
 }
 
@@ -652,12 +525,12 @@ int bb_gemm_tc_run(const TcGemmArgs& G0, cudaStream_t s) {
                         G.b[0].mode == TC_WDGRAD;
   G.lut_k = need_lut ? (int)G.K : 0;
   if (G.lut_k > kMaxLutK) return BB_ERR_UNSUPPORTED;
-  // Two register budgets are compiled: 1 CTA/SM (156 registers, no spills) and 2 CTAs/SM (capped at 96, a few
-  // spilled words).  Measured on B200: the convolution gathers are issue-latency bound and gain ~20 % from the
-  // second resident CTA (implicit_maml N=800: 16.7 -> 20.2 it/s); plain strided GEMMs are ~3 % faster with 1.
+  // Two register budgets are compiled: 1 CTA/SM and, for 64-wide tiles, 2 CTAs/SM (capped at 128 registers).  The convolution gathers
+  // are issue-latency bound and gain from a second resident CTA; plain strided GEMMs keep the larger budget.
   static const int forced = getenv("BB200_TC_OCC") ? atoi(getenv("BB200_TC_OCC")) : 0;
   const int occ = forced ? forced : (need_lut || G.a[0].mode == TC_PIXK ? 2 : 1);
-  if (occ >= 2) return bn == 64 ? launch_tc<64, 2>(G, ksplit, s) : launch_tc<128, 2>(G, ksplit, s);
+  // (128 accumulator registers of a 128-wide tile do not fit the 2-CTA budget: those tiles always run one per SM)
+  if (occ >= 2 && bn == 64) return launch_tc<64, 2>(G, ksplit, s);
   return bn == 64 ? launch_tc<64, 1>(G, ksplit, s) : launch_tc<128, 1>(G, ksplit, s);
 }
 

@@ -1,4 +1,4 @@
-// Argument block of the tcgen05 dual-product GEMM / implicit-GEMM convolution kernel (gemm_tc.cu).
+// Argument block of the wgmma dual-product GEMM / implicit-GEMM convolution kernel (gemm_tc.cu).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

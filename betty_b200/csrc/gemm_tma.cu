@@ -1,23 +1,22 @@
 // K5/K6 tensor-core path, TMA-fed: dual-product GEMM and stride-1 convolution (forward / input-gradient form) on
-// tcgen05.mma with operands brought into shared memory by the TMA unit.
+// wgmma.mma_async with operands brought into shared memory by the TMA unit.
 //
 //   D[m][n] (beta/atomic)= sum over up to two operand pairs p of  sum_k A_p[m][k] * B_p[n][k]   (+ bias[n])
 //
-// The software-staged kernel in gemm_tc.cu spends >95 % of its time in the producer warps (address arithmetic,
-// 4-byte gathers, bf16 conversion, swizzled stores; ncu: tensor pipe ~1 %).  Here every operand is first made
-// TMA-addressable -- bf16, unit stride along one matrix dimension, 16-byte aligned rows; base activations and
-// autocast weight copies already are, tangents / adjoints (fp32 arena slices) go through a streaming pack kernel --
-// and one elected thread issues cp.async.bulk.tensor loads that land in the SWIZZLE_128B layout the UMMA
-// descriptors read:
+// The software-staged kernel in gemm_tc.cu spends most of its time staging operands (address arithmetic, 4-byte
+// gathers, bf16 conversion, swizzled stores).  Here every operand is first made TMA-addressable -- bf16, unit stride
+// along one matrix dimension, 16-byte aligned rows; base activations and autocast weight copies already are,
+// tangents / adjoints (fp32 arena slices) go through a streaming pack kernel -- and one elected thread issues
+// cp.async.bulk.tensor loads that land in the SWIZZLE_128B layout the wgmma descriptors read:
 //   K-major operand  (k contiguous in memory): one box of 64 k x ROWS rows      -> rows of 128 B
 //   MN-major operand (m/n contiguous):         ROWS/64 boxes of 64 mn x 64 k    -> 8x64 atoms, SBO 1024 B, LBO 8 KB
 //   convolution A    (NHWC bf16 activations):  one 4-D box 64 ch x Wb x Hb x 1 per (tap, channel block); the
 //                    window displacement is a coordinate offset, zero padding is TMA out-of-bounds fill
 // so transposed views cost nothing and an implicit-GEMM convolution is nine shifted box loads per 64 channels.
 //
-// Roles (192 threads): warp 0 = TMA producer (one lane), warp 1 = TMEM alloc + MMA issue (one lane), warps 2-5 =
-// epilogue (tcgen05.ld 32 lanes x 32 columns, warp w owns TMEM lanes 32*(w%4)..).  3-4 stage mbarrier ring; two
-// CTAs per SM so one CTA's epilogue overlaps the other's main loop.
+// Roles (288 threads): warps 0-7 = two consumer warpgroups (warpgroup g issues wgmma m64nBNk16 for rows 64g..64g+63
+// of the 128-row tile and stores them from its registers), warp 8 = TMA producer (one lane).  3-8 stage mbarrier
+// ring; two CTAs per SM on full grids so one CTA's epilogue overlaps the other's main loop.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -35,13 +34,15 @@
 
 thread_local BbScratch bb_scratch = {nullptr, 0, 0};
 thread_local uint64_t bb_scratch_gen = 0;
+thread_local BbReduceWs bb_reduce_ws = {nullptr, 0};
 
 namespace {
 
 using namespace bbtc;
 
 constexpr int BM = 128, BK = 64;
-constexpr int NTHREADS = 192;
+constexpr int NTHREADS = 288;
+constexpr int PRODUCER_WARP = 8;
 constexpr int A_TILE = BM * BK * 2;   // 16 KB
 
 constexpr int MAX_STAGES = 8;
@@ -55,81 +56,118 @@ struct Cfg {
   static constexpr size_t smem(int stages) { return (size_t)stages * kStage + 1024 + 256; }
 };
 
-// Epilogue store of one 32-column chunk of a thread's accumulator row.  Written for a low instruction count: the
-// epilogue warps are four single warps per CTA, so their time is (instructions x dependent-issue latency), not
-// bandwidth -- the first version spent ~30 integer instructions per stored value on 64-bit index arithmetic and
-// per-element predicates (ncu source page: 7.7 us per 128x64 tile, see profiles/r01_persist_ncu.md).  Here every mode
-// decision is made once per chunk and addresses advance by pointer increments.
-__device__ __forceinline__ void epi_store(const TmaGemmArgs& G, uint32_t (&v)[32], float* dst, int64_t col_stride, int col0,
-                                          bool add_bias, bool vec, bool vec_red) {
-  const int ncols = (G.N - col0) < 32 ? (int)(G.N - col0) : 32;
-  const bool full = ncols == 32;
-  if (add_bias) {
-    const float* bp = G.bias + (int64_t)col0 * G.bias_stride;
-    if (full && G.bias_stride == 1 && (reinterpret_cast<uintptr_t>(bp) & 15) == 0) {
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b = *reinterpret_cast<const float4*>(bp + j);
-        v[j] = __float_as_uint(__uint_as_float(v[j]) + b.x);
-        v[j + 1] = __float_as_uint(__uint_as_float(v[j + 1]) + b.y);
-        v[j + 2] = __float_as_uint(__uint_as_float(v[j + 2]) + b.z);
-        v[j + 3] = __float_as_uint(__uint_as_float(v[j + 3]) + b.w);
-      }
+// Where the rows of an output tile go: row r (0..127) of the tile -> base offset, column stride, validity.
+struct OutRows {
+  int omode, img, h0;
+  int64_t m0, bz;
+  __device__ __forceinline__ bool map(const TmaGemmArgs& G, int r, int64_t* base, int64_t* col_stride) const {
+    if (omode == 1) {
+      const int64_t q = (int64_t)h0 * G.Wb + r;   // Wb == output width
+      *base = (int64_t)img * G.OCH * G.OHW + q;
+      *col_stride = G.OHW;
+      return r < G.Wb * G.Hb && q < G.OHW;
+    }
+    const int64_t row = m0 + r;
+    if (omode == 2) {
+      const int64_t im = row / G.OHW;
+      *base = im * G.OCH * G.OHW + (row - im * G.OHW);
+      *col_stride = G.OHW;
     } else {
-#pragma unroll
-      for (int j = 0; j < 32; ++j)
-        if (j < ncols) v[j] = __float_as_uint(__uint_as_float(v[j]) + bp[(int64_t)j * G.bias_stride]);
+      *base = bz * G.obs + row * G.ors;
+      *col_stride = G.ocs;
     }
+    return row < G.M;
   }
-  if (full && vec) {
+};
+
+// Epilogue of one warpgroup's 64 x BN accumulator fragment (d[4j + 2h + e] = row frag_row + 8h, column
+// 8j + frag_col + e).  Mode decisions are made once per row; row-major fp32 outputs are written as float2.
+template <int BN_>
+__device__ __forceinline__ void epi_store(const TmaGemmArgs& G, const float (&acc)[BN_ / 2], const OutRows& R, int wg, int t,
+                                          int n0, bool add_bias) {
+  const bool vec = G.omode == 0 && G.ocs == 1 && (G.ors & 1) == 0 && (G.obs & 1) == 0 &&
+                   ((reinterpret_cast<uintptr_t>(G.out) & 7) == 0) && G.ksplit == 1;
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      float4 o = make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                             __uint_as_float(v[j + 3]));
-      float4* q = reinterpret_cast<float4*>(dst + j);
-      if (G.beta) {
-        const float4 old = *q;
-        o.x += old.x; o.y += old.y; o.z += old.z; o.w += old.w;
+  for (int h = 0; h < 2; ++h) {
+    int64_t base, cs;
+    if (!R.map(G, wg * 64 + frag_row(t) + 8 * h, &base, &cs)) continue;
+#pragma unroll
+    for (int j = 0; j < BN_ / 8; ++j) {
+      const int col = n0 + 8 * j + frag_col(t);
+      if (col >= G.N) continue;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      const bool two = col + 1 < G.N;
+      if (add_bias) {
+        v0 += G.bias[(int64_t)col * G.bias_stride];
+        if (two) v1 += G.bias[(int64_t)(col + 1) * G.bias_stride];
       }
-      *q = o;
+      float* q = G.out + base + (int64_t)col * cs;
+      if (vec && two) {
+        float2* q2 = reinterpret_cast<float2*>(q);
+        float2 o = make_float2(v0, v1);
+        if (G.beta) {
+          const float2 old = *q2;
+          o.x += old.x; o.y += old.y;
+        }
+        *q2 = o;
+      } else if (G.ksplit > 1) {
+        atomicAdd(q, v0);
+        if (two) atomicAdd(q + cs, v1);
+      } else if (G.beta) {
+        *q += v0;
+        if (two) q[cs] += v1;
+      } else {
+        *q = v0;
+        if (two) q[cs] = v1;
+      }
     }
-    return;
   }
-  if (full && vec_red) {
-    // split-K partial sums: 128-bit reductions (red.global.add.v4.f32), a quarter of the atomic traffic
-#pragma unroll
-    for (int j = 0; j < 32; j += 4)
-      asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(dst + j), "f"(__uint_as_float(v[j])),
-                   "f"(__uint_as_float(v[j + 1])), "f"(__uint_as_float(v[j + 2])), "f"(__uint_as_float(v[j + 3]))
-                   : "memory");
-    return;
+}
+
+// TMA loads of k-block `it` of a tile into stage buffer sa / sb (one elected producer thread)
+template <int BN_>
+__device__ __forceinline__ void produce(const TmaGemmArgs& G, int pair, int kb, uint32_t sa, uint32_t sb, uint32_t bar,
+                                        int m0, int n0, int img, int h0, int bz) {
+  const int k0 = kb * BK;
+  mbar_expect_tx(bar, G.a_bytes + G.b_bytes);
+  const int ak = G.a_kind[pair];
+  if (ak == TMA_KMAJ) {
+    tma_load_3d(sa, &G.a[pair], bar, k0, m0, bz);
+  } else if (ak == TMA_MNMAJ) {
+    tma_load_3d(sa, &G.a[pair], bar, m0, k0, bz);
+    tma_load_3d(sa + 8192, &G.a[pair], bar, m0 + 64, k0, bz);
+  } else {
+    const int tap = kb / G.cblocks, cb = kb - tap * G.cblocks;
+    const int i = tap / G.KW, j = tap - i * G.KW;
+    const int dy = G.flip ? G.ph - i : i - G.ph, dx = G.flip ? G.pw - j : j - G.pw;
+    tma_load_4d(sa, &G.a[pair], bar, cb * 64, dx, h0 + dy, img);
   }
-  float* q = dst;
-  if (G.ksplit > 1) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      if (j < ncols) atomicAdd(q, __uint_as_float(v[j]));
-      q += col_stride;
-    }
-  } else if (G.beta) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      if (j < ncols) *q += __uint_as_float(v[j]);
-      q += col_stride;
-    }
-  } else if (full) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      *q = __uint_as_float(v[j]);
-      q += col_stride;
-    }
+  const int bzb = ak == TMA_CONV ? 0 : bz;
+  if (G.b_kind[pair] == TMA_KMAJ) {
+    tma_load_3d(sb, &G.b[pair], bar, k0, n0, bzb);
   } else {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      if (j < ncols) *q = __uint_as_float(v[j]);
-      q += col_stride;
-    }
+    for (int q = 0; q < BN_ / 64; ++q) tma_load_3d(sb + q * 8192, &G.b[pair], bar, n0 + q * 64, k0, bzb);
   }
+}
+
+// The MMAs of one k-block for this warpgroup's 64 rows; the previous k-block's stage is handed back once its MMAs
+// have retired (wait_group 1), so one stage per warpgroup stays in flight.
+template <int BN_>
+__device__ __forceinline__ void consume(const TmaGemmArgs& G, float (&acc)[BN_ / 2], int pair, uint32_t a_addr, uint32_t b_addr,
+                                        bool first) {
+  const bool a_mn = G.a_kind[pair] == TMA_MNMAJ, b_mn = G.b_kind[pair] == TMA_MNMAJ;
+  fence_acc(acc);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < BK / 16; ++k) {
+    const uint64_t da = a_mn ? desc_mn(a_addr + k * 2048, 8192) : desc_k(a_addr + k * 32);
+    const uint64_t db = b_mn ? desc_mn(b_addr + k * 2048, 8192) : desc_k(b_addr + k * 32);
+    wgmma_bf16<BN_>(acc, da, db, (!first || k > 0) ? 1u : 0u, a_mn, b_mn);
+  }
+  wgmma_commit();
+  fence_acc(acc);
+  wgmma_wait<1>();
 }
 
 template <int BN_>
@@ -139,10 +177,9 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_kernel(const __grid_cons
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::kStage);
-  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + MAX_STAGES), accum = smem_u32(bars + 2 * MAX_STAGES);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 1);
+  const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + MAX_STAGES);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int n0 = blockIdx.x * BN_;
   const int bz = blockIdx.z / G.ksplit;            // batch index (ksplit == 1 when batched)
   const int split = blockIdx.z - bz * G.ksplit;
@@ -166,18 +203,13 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_kernel(const __grid_cons
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 2);   // one arrival per consumer warpgroup
     }
-    mbar_init(accum, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), (uint32_t)BN_);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ---------------- TMA producer ----------------
     if (elect_one()) {
       for (int p = 0; p < G.npairs; ++p) {
@@ -188,115 +220,35 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_kernel(const __grid_cons
         const int s = it % STAGES;
         if (it >= STAGES) mbar_wait(empty0 + 8 * s, ((it / STAGES) - 1) & 1);
         const int pair = it / nkb;
-        const int kb = (int)kb_beg + (it - pair * nkb);
-        const int k0 = kb * BK;
-        const uint32_t bar = full0 + 8 * s;
-        const uint32_t sa = smem_u32(smem + s * C::kStage), sb = sa + A_TILE;
-        mbar_expect_tx(bar, G.a_bytes + G.b_bytes);
-        const int ak = G.a_kind[pair];
-        if (ak == TMA_KMAJ) {
-          tma_load_3d(sa, &G.a[pair], bar, k0, m0, bz);
-        } else if (ak == TMA_MNMAJ) {
-          tma_load_3d(sa, &G.a[pair], bar, m0, k0, bz);
-          tma_load_3d(sa + 8192, &G.a[pair], bar, m0 + 64, k0, bz);
-        } else {
-          const int tap = kb / G.cblocks, cb = kb - tap * G.cblocks;
-          const int i = tap / G.KW, j = tap - i * G.KW;
-          const int dy = G.flip ? G.ph - i : i - G.ph, dx = G.flip ? G.pw - j : j - G.pw;
-          tma_load_4d(sa, &G.a[pair], bar, cb * 64, dx, h0 + dy, img);
-        }
-        const int bzb = ak == TMA_CONV ? 0 : bz;
-        if (G.b_kind[pair] == TMA_KMAJ) {
-          tma_load_3d(sb, &G.b[pair], bar, k0, n0, bzb);
-        } else {
-#pragma unroll
-          for (int q = 0; q < BN_ / 64; ++q) tma_load_3d(sb + q * 8192, &G.b[pair], bar, n0 + q * 64, k0, bzb);
-        }
+        const uint32_t sa = smem_u32(smem + s * C::kStage);
+        produce<BN_>(G, pair, (int)kb_beg + (it - pair * nkb), sa, sa + A_TILE, full0 + 8 * s, m0, n0, img, h0, bz);
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer ----------------
-    if (elect_one()) {
-      for (int it = 0; it < total_kb; ++it) {
-        const int s = it % STAGES;
-        const int pair = it / nkb;
-        const bool a_mn = G.a_kind[pair] == TMA_MNMAJ, b_mn = G.b_kind[pair] == TMA_MNMAJ;
-        const uint32_t idesc = idesc_bf16(BM, BN_, a_mn, b_mn);
-        mbar_wait(full0 + 8 * s, (it / STAGES) & 1);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * C::kStage), b_addr = a_addr + A_TILE;
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k) {
-          const uint64_t da = a_mn ? desc_mn(a_addr + k * 2048, 8192) : desc_k(a_addr + k * 32);
-          const uint64_t db = b_mn ? desc_mn(b_addr + k * 2048, 8192) : desc_k(b_addr + k * 32);
-          umma_bf16(tmem_base, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(empty0 + 8 * s);
-      }
-      if (total_kb > 0) umma_commit(accum);
-    }
-    __syncwarp();
   } else {
-    // ---------------- epilogue (warps 2..5) ----------------
-    if (total_kb > 0) {
-      mbar_wait(accum, 0, 100);
-      tc_fence_after();
-    }
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    bool row_ok;
-    int64_t row_base, col_stride;
-    if (G.omode == 1) {
-      const int64_t q = (int64_t)h0 * G.Wb + r;   // Wb == output width
-      row_ok = r < G.Wb * G.Hb && q < G.OHW;
-      row_base = (int64_t)img * G.OCH * G.OHW + q;
-      col_stride = G.OHW;
-    } else if (G.omode == 2) {
-      const int64_t row = (int64_t)m0 + r;
-      row_ok = row < G.M;
-      const int64_t im = row / G.OHW;
-      row_base = im * G.OCH * G.OHW + (row - im * G.OHW);
-      col_stride = G.OHW;
-    } else {
-      const int64_t row = (int64_t)m0 + r;
-      row_ok = row < G.M;
-      row_base = (int64_t)bz * G.obs + row * G.ors;
-      col_stride = G.ocs;
-    }
-    const bool row_vec = G.omode == 0 && G.ocs == 1 && (G.ors & 3) == 0 && (G.obs & 3) == 0 &&
-                         ((reinterpret_cast<uintptr_t>(G.out) & 15) == 0);
-    const bool vec = row_vec && G.ksplit == 1, vec_red = row_vec && G.ksplit > 1;
-#pragma unroll 1
-    for (int c = 0; c < BN_ / 32; ++c) {
-      uint32_t v[32];
-      if (total_kb > 0) {
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(c * 32), v);
-      } else {
+    // ---------------- consumers (warpgroups 0, 1) ----------------
+    const int wg = tid >> 7, t = tid & 127;
+    float acc[BN_ / 2];
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0u;
-      }
-      if (!row_ok) continue;
-      const int col0 = n0 + c * 32;
-      if (col0 >= G.N) continue;
-      epi_store(G, v, G.out + row_base + (int64_t)col0 * col_stride, col_stride, col0, G.bias != nullptr && split == 0, vec,
-                vec_red);
+    for (int i = 0; i < BN_ / 2; ++i) acc[i] = 0.f;
+    for (int it = 0; it < total_kb; ++it) {
+      const int s = it % STAGES;
+      mbar_wait(full0 + 8 * s, (it / STAGES) & 1);
+      const uint32_t a_addr = smem_u32(smem + s * C::kStage);
+      consume<BN_>(G, acc, it / nkb, a_addr + (uint32_t)wg * 8192u, a_addr + A_TILE, it == 0);
+      if (it > 0 && t == 0) mbar_arrive(empty0 + 8 * ((it - 1) % STAGES));
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)BN_);
+    wgmma_wait<0>();
+    fence_acc(acc);
+    const OutRows R{G.omode, img, h0, (int64_t)m0, (int64_t)bz};
+    epi_store<BN_>(G, acc, R, wg, t, n0, G.bias != nullptr && split == 0);
   }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
 // Persistent variant for launches with many more tiles than SMs (convolutions: one tile per 128 pixels).  A CTA
-// walks tiles blockIdx.x, +gridDim.x, ...; the TMA producer and the MMA warp run ahead across tile boundaries on the
-// same stage ring, and the accumulator is double-buffered in TMEM (2 x BN columns) so the epilogue of tile i
-// (tcgen05.ld + global stores) overlaps the loads and MMAs of tile i+1.  The one-tile-per-CTA kernel above pays
-// barrier init + TMEM allocation + a cold TMA round trip per tile (~4-8 us for a 1-9 k-block tile).
-//   barriers: full[S] / empty[S] (stage ring), acc_full[2] (MMA -> epilogue), acc_empty[2] (4 epilogue warps -> MMA)
+// walks tiles blockIdx.x, +gridDim.x, ...; the TMA producer runs ahead across tile boundaries on the same stage ring,
+// so the loads of tile i+1 overlap the epilogue of tile i (register accumulators: the consumers store a tile, then
+// start the next).  The one-tile-per-CTA kernel above pays barrier init and a cold TMA round trip per tile.
 // No split-K, no batch (conv and plane-output GEMMs only).
 template <int BN_>
 __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_persist_kernel(const __grid_constant__ TmaGemmArgs G, int ntiles_n,
@@ -307,10 +259,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_persist_kernel(const __g
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * C::kStage);
   const uint32_t full0 = smem_u32(bars), empty0 = smem_u32(bars + MAX_STAGES);
-  const uint32_t accf0 = smem_u32(bars + 2 * MAX_STAGES), acce0 = smem_u32(bars + 2 * MAX_STAGES + 2);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 4);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int nkb = (int)((G.K + BK - 1) / BK);
   const int per_tile = nkb * G.npairs;
   const bool conv = G.a_kind[0] == TMA_CONV;
@@ -318,21 +268,13 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_persist_kernel(const __g
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(accf0 + 8 * b, 1);
-      mbar_init(acce0 + 8 * b, 4);
+      mbar_init(empty0 + 8 * s, 2);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_slot), (uint32_t)(2 * BN_));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (warp == PRODUCER_WARP) {
     // ---------------- TMA producer ----------------
     if (elect_one()) {
       for (int p = 0; p < G.npairs; ++p) {
@@ -352,113 +294,36 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_persist_kernel(const __g
         for (int it = 0; it < per_tile; ++it, ++git) {
           const int s = git % STAGES;
           if (git >= STAGES) mbar_wait(empty0 + 8 * s, ((git / STAGES) - 1) & 1);
-          const int pair = it / nkb, kb = it - pair * nkb, k0 = kb * BK;
-          const uint32_t bar = full0 + 8 * s;
-          const uint32_t sa = smem_u32(smem + s * C::kStage), sb = sa + A_TILE;
-          mbar_expect_tx(bar, G.a_bytes + G.b_bytes);
-          const int ak = G.a_kind[pair];
-          if (ak == TMA_KMAJ) {
-            tma_load_3d(sa, &G.a[pair], bar, k0, m0, 0);
-          } else if (ak == TMA_MNMAJ) {
-            tma_load_3d(sa, &G.a[pair], bar, m0, k0, 0);
-            tma_load_3d(sa + 8192, &G.a[pair], bar, m0 + 64, k0, 0);
-          } else {
-            const int tap = kb / G.cblocks, cb = kb - tap * G.cblocks;
-            const int i = tap / G.KW, j = tap - i * G.KW;
-            const int dy = G.flip ? G.ph - i : i - G.ph, dx = G.flip ? G.pw - j : j - G.pw;
-            tma_load_4d(sa, &G.a[pair], bar, cb * 64, dx, h0 + dy, img);
-          }
-          if (G.b_kind[pair] == TMA_KMAJ) {
-            tma_load_3d(sb, &G.b[pair], bar, k0, n0, 0);
-          } else {
-#pragma unroll
-            for (int q = 0; q < BN_ / 64; ++q) tma_load_3d(sb + q * 8192, &G.b[pair], bar, n0 + q * 64, k0, 0);
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer ----------------
-    if (elect_one()) {
-      int git = 0, lt = 0;   // lt = this CTA's tile counter
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-        const int buf = lt & 1;
-        if (lt >= 2) {   // the epilogue must have drained this accumulator (tile lt-2)
-          mbar_wait(acce0 + 8 * buf, ((lt >> 1) - 1) & 1);
-          tc_fence_after();
-        }
-        const uint32_t tacc = tmem_base + (uint32_t)(buf * BN_);
-        for (int it = 0; it < per_tile; ++it, ++git) {
-          const int s = git % STAGES;
           const int pair = it / nkb;
-          const bool a_mn = G.a_kind[pair] == TMA_MNMAJ, b_mn = G.b_kind[pair] == TMA_MNMAJ;
-          const uint32_t idesc = idesc_bf16(BM, BN_, a_mn, b_mn);
-          mbar_wait(full0 + 8 * s, (git / STAGES) & 1);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * C::kStage), b_addr = a_addr + A_TILE;
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t da = a_mn ? desc_mn(a_addr + k * 2048, 8192) : desc_k(a_addr + k * 32);
-            const uint64_t db = b_mn ? desc_mn(b_addr + k * 2048, 8192) : desc_k(b_addr + k * 32);
-            umma_bf16(tacc, da, db, idesc, (it > 0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(empty0 + 8 * s);
+          const uint32_t sa = smem_u32(smem + s * C::kStage);
+          produce<BN_>(G, pair, it - pair * nkb, sa, sa + A_TILE, full0 + 8 * s, m0, n0, img, h0, 0);
         }
-        umma_commit(accf0 + 8 * buf);
       }
     }
-    __syncwarp();
   } else {
-    // ---------------- epilogue (warps 2..5) ----------------
-    const int quarter = warp & 3;
-    const int r = quarter * 32 + lane;
-    const bool vec = G.omode == 0 && G.ocs == 1 && (G.ors & 3) == 0 && ((reinterpret_cast<uintptr_t>(G.out) & 15) == 0);
-    int lt = 0;
-    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++lt) {
-      const int buf = lt & 1;
+    // ---------------- consumers ----------------
+    const int wg = tid >> 7, t = tid & 127;
+    float acc[BN_ / 2];
+    int git = 0;
+    for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const int mt = tile / ntiles_n, n0 = (tile - mt * ntiles_n) * BN_;
-      bool row_ok;
-      int64_t row_base, col_stride;
-      if (G.omode == 1) {
-        const int img = mt / G.tiles_per_img, h0 = (mt - img * G.tiles_per_img) * G.Hb;
-        const int64_t q = (int64_t)h0 * G.Wb + r;
-        row_ok = r < G.Wb * G.Hb && q < G.OHW;
-        row_base = (int64_t)img * G.OCH * G.OHW + q;
-        col_stride = G.OHW;
-      } else if (G.omode == 2) {
-        const int64_t row = (int64_t)mt * BM + r;
-        row_ok = row < G.M;
-        const int64_t im = row / G.OHW;
-        row_base = im * G.OCH * G.OHW + (row - im * G.OHW);
-        col_stride = G.OHW;
-      } else {
-        const int64_t row = (int64_t)mt * BM + r;
-        row_ok = row < G.M;
-        row_base = row * G.ors;
-        col_stride = G.ocs;
+      for (int it = 0; it < per_tile; ++it, ++git) {
+        const int s = git % STAGES;
+        mbar_wait(full0 + 8 * s, (git / STAGES) & 1);
+        const uint32_t a_addr = smem_u32(smem + s * C::kStage);
+        consume<BN_>(G, acc, it / nkb, a_addr + (uint32_t)wg * 8192u, a_addr + A_TILE, it == 0);
+        if (it > 0 && t == 0) mbar_arrive(empty0 + 8 * ((git - 1) % STAGES));
       }
-      mbar_wait(accf0 + 8 * buf, (lt >> 1) & 1, 60);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < BN_ / 32; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * BN_ + c * 32), v);
-        if (c == BN_ / 32 - 1) {   // last read of this accumulator: hand it back to the MMA warp before storing
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(acce0 + 8 * buf);
-        }
-        const int col0 = n0 + c * 32;
-        if (!row_ok || col0 >= G.N) continue;
-        epi_store(G, v, G.out + row_base + (int64_t)col0 * col_stride, col_stride, col0, G.bias != nullptr, vec, false);
+      wgmma_wait<0>();
+      fence_acc(acc);
+      if (t == 0) mbar_arrive(empty0 + 8 * ((git - 1) % STAGES));
+      OutRows R{G.omode, 0, 0, (int64_t)mt * BM, 0};
+      if (conv) {
+        R.img = mt / G.tiles_per_img;
+        R.h0 = (mt - R.img * G.tiles_per_img) * G.Hb;
       }
+      epi_store<BN_>(G, acc, R, wg, t, n0, G.bias != nullptr);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)(2 * BN_));
   }
 }
 
@@ -871,7 +736,7 @@ int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* 
     if (M < 64 || N < min_n || K < 8) return BB_DECLINED;
     if (K < 64 && min_n >= 64) return BB_DECLINED;
   } else {
-    // batched (attention score / context products): the tiles are mostly padding, but a 128 x 64 tcgen05 tile costs
+    // batched (attention score / context products): the tiles are mostly padding, but a 128 x 64 wgmma tile costs
     // less than the SIMT kernel's inner loop as soon as the products are not tiny
     if (M < 32 || N < 32 || K < 32 || batch > 65535 || plane_ohw > 0 || bias != nullptr) return BB_DECLINED;
   }
@@ -885,10 +750,9 @@ int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* 
   }
   alignas(64) TmaGemmArgs G;
   memset(&G, 0, sizeof(G));
-  // Tile width and split-K by a cost model.  The kernel is bound by what one SM can pull through the TMA unit
-  // (measured ~43 B/clk/SM = the chip's ~6300 B/clk L2 throughput / 148; a 128 x bn x 64 k-block costs 16 + bn/8 KB),
-  // so the time of a configuration is (waves of CTAs) x (k-blocks per CTA) x (bytes per k-block) / per-SM rate; split-K
-  // adds a memset launch and the reduction traffic of its partial tiles.
+  // Tile width and split-K by a cost model.  The kernel is bound by what one SM can pull through the TMA unit (a
+  // 128 x bn x 64 k-block costs 16 + bn/8 KB), so the time of a configuration is (waves of CTAs) x (k-blocks per CTA)
+  // x (bytes per k-block) / per-SM rate; split-K adds a memset launch and the reduction traffic of its partial tiles.
   const int64_t mtiles = (M + BM - 1) / BM;
   const int64_t kblocks = (K + BK - 1) / BK;
   const bool can_split = batch == 1 && plane_ohw == 0 && (beta || out_dense) && kblocks >= 8;

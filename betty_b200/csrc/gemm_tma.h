@@ -1,4 +1,4 @@
-// TMA-fed tcgen05 dual-product GEMM / 3x3-style convolution (gemm_tma.cu, conv_tma.cu).
+// TMA-fed wgmma dual-product GEMM / 3x3-style convolution (gemm_tma.cu, conv_tma.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>

@@ -17,7 +17,7 @@ namespace {
 
 constexpr int kThreads = 512;
 constexpr int kBlocksPerSM = 4;
-constexpr int kMaxGrid = BB_SM_COUNT * kBlocksPerSM;  // 592 persistent-ish blocks, grid-stride
+constexpr int kMaxGrid = BB_SM_COUNT * kBlocksPerSM;  // 528 persistent-ish blocks, grid-stride
 
 inline int grid_for(int64_t n4) {
   int64_t want = (n4 + kThreads - 1) / kThreads;

@@ -17,6 +17,7 @@ struct bb_plan {
   int launches[3] = {0, 0, 0};
   void* scratch = nullptr;      // bf16 operand packs of the TMA-fed tensor-core path (tma.h)
   int64_t scratch_bytes = 0;
+  float* reduce_ws = nullptr;   // fixed-order reductions of the node launchers (tma.h BbReduceWs), allocated on first run
   uint8_t* persist = nullptr;   // plan-lifetime packs of K-loop constants, bump-allocated per node
   int64_t persist_bytes = 0, persist_used = 0;
   std::vector<void*> node_persist;
@@ -116,9 +117,27 @@ int dispatch(const bb_node& nd, int pass, cudaStream_t s) {
   }
 }
 
+// 24 MB holds the per-CTA weight-gradient partials of a 64 -> 64 channel 3x3 convolution on every SM (132 x 144 KB) and
+// the split-K partials of the SIMT products; launchers split less when a reduction would not fit.
+constexpr size_t kReduceWsBytes = 24u << 20;
+
+// Allocated by the first pass, which runs eagerly before any K-loop capture.
+cudaError_t publish_reduce_ws(bb_plan* p) {
+  if (p->reduce_ws == nullptr) {
+    const cudaError_t e = cudaMalloc(&p->reduce_ws, kReduceWsBytes);
+    if (e != cudaSuccess) {
+      p->reduce_ws = nullptr;
+      return e;
+    }
+  }
+  bb_reduce_ws = BbReduceWs{p->reduce_ws, kReduceWsBytes};
+  return cudaSuccess;
+}
+
 int run_pass(bb_plan* p, int pass, cudaStream_t s, bool in_loop = false) {
   if (pass < 0 || pass > 2) return BB_ERR_ARG;
   const int skip = in_loop ? p->shift_node : -1;
+  BB_CUDA_TRY(publish_reduce_ws(p));
   bb_scratch = BbScratch{reinterpret_cast<uint8_t*>(p->scratch), (size_t)p->scratch_bytes, 0};
   bb_scratch_reset();
   const int tally0 = bb_launch_tally;
@@ -201,6 +220,10 @@ int bb_plan_create(const struct bb_node* nodes, int n_nodes, bb_plan** out) {
 }
 
 int bb_plan_destroy(bb_plan* plan) {
+  if (plan && plan->reduce_ws) {
+    if (bb_reduce_ws.base == plan->reduce_ws) bb_reduce_ws = BbReduceWs{nullptr, 0};
+    cudaFree(plan->reduce_ws);
+  }
   delete plan;
   return BB_OK;
 }
@@ -243,6 +266,7 @@ int bb_plan_graph_captures(const bb_plan* plan) { return plan ? plan->graph_capt
 int bb_plan_node_route(bb_plan* plan, int node, int pass) {
   // introspection for the unit tests: 2 = TMA-fed tensor-core convolution path takes (node, pass), 0 = another path
   if (!plan || node < 0 || node >= (int)plan->nodes.size()) return BB_ERR_ARG;
+  BB_CUDA_TRY(publish_reduce_ws(plan));
   bb_scratch = BbScratch{reinterpret_cast<uint8_t*>(plan->scratch), (size_t)plan->scratch_bytes, 0};
   const bb_node& nd = plan->nodes[node];
   if (nd.op == BB_OP_CONV2D && bb_conv_tma_ok(nd, pass)) return 2;
@@ -293,6 +317,7 @@ int bb_plan_hvp_replay(bb_plan* plan, void* stream) {
 int bb_plan_profile(bb_plan* plan, int pass, float* ms_per_node, void* stream) {
   if (!plan || pass < 0 || pass > 2 || !ms_per_node) return BB_ERR_ARG;
   cudaStream_t s = (cudaStream_t)stream;
+  BB_CUDA_TRY(publish_reduce_ws(plan));
   bb_scratch = BbScratch{reinterpret_cast<uint8_t*>(plan->scratch), (size_t)plan->scratch_bytes, 0};
   bb_scratch_reset();
   const int n = (int)plan->nodes.size();
@@ -353,6 +378,6 @@ int bb_plan_cg_loop(bb_plan* plan, int iterations, float cg_alpha, float* x, flo
   });
 }
 
-const char* bb_version(void) { return "betty_b200 0.1.0 (sm_100a)"; }
+const char* bb_version(void) { return "betty_b200 0.1.0 (sm_90a)"; }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
-// Inline-PTX wrappers shared by the TMA-fed tcgen05 kernels: mbarrier, TMA tensor loads, UMMA descriptors,
-// tcgen05.mma / commit / ld, TMEM allocation.
+// Inline-PTX wrappers shared by the tensor-core kernels: mbarrier, TMA tensor loads, wgmma descriptors and
+// wgmma.mma_async / commit / wait (sm_90a).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -36,8 +36,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, unsigne
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // TMA: global (tensor map) -> shared, completion on an mbarrier (complete_tx::bytes)
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
@@ -64,75 +62,92 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map)) : "memory");
 }
 
-// tcgen05.mma kind::f16 (bf16 operands from shared memory descriptors, fp32 accumulator in TMEM)
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// one thread of a converged warp; unlike `lane == 0` the compiler treats the guarded region as warp-uniform, so the
-// tcgen05.mma operands stay in uniform registers (no R2UR + ELECT/BRA.U.ANY loop around every instruction)
+// one thread of a converged warp; unlike `lane == 0` the compiler treats the guarded region as warp-uniform
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n.reg .pred p;\nelect.sync _|p, 0xffffffff;\nselp.u32 %0, 1, 0, p;\n}\n" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
-// Shared-memory matrix descriptors, SWIZZLE_128B (layout type 2), descriptor version 1, 8-row groups 1024 B apart.
+// Shared-memory matrix descriptors of wgmma (sm_90a), SWIZZLE_128B (layout type 1 at bit 62), 8-row groups 1024 B apart.
 //   K-major:  rows of 64 bf16 (128 B); LBO unused (1).
 //   MN-major: atom = 8 k-rows x 64 mn; atoms of one 64-wide mn block consecutive along k (SBO 1024 B), the next
 //             mn block starts lbo_bytes later.
+// The swizzle is a function of the shared-memory address bits, so a descriptor may start on any 16-byte column or
+// 128-byte row of a 1024-byte-aligned buffer with base offset 0.
+constexpr uint64_t kDescSw128 = (uint64_t)1 << 62;
 __device__ __forceinline__ uint64_t desc_k(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)1 << 16) | ((uint64_t)(1024 >> 4) << 32) | kDescSw128;
 }
 __device__ __forceinline__ uint64_t desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);
-  d |= (uint64_t)(lbo_bytes >> 4) << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// instruction descriptor: D fp32, A/B bf16, M x N tile, optional MN-major operands
-__host__ __device__ constexpr uint32_t idesc_bf16(int M, int N, bool a_mn, bool b_mn) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn ? (1u << 15) : 0u) | (b_mn ? (1u << 16) : 0u) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) |
+         kDescSw128;
 }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t slot_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(slot_smem), "r"(cols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t base, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(base), "r"(cols));
+// keeps the compiler from moving accumulator reads / writes across the asynchronous wgmma window
+template <int R>
+__device__ __forceinline__ void fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = lane)
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
+
+// wgmma.mma_async m64nNk16, bf16 operands from shared-memory descriptors, fp32 accumulators in registers of the
+// issuing warpgroup; TA / TB = 1: the operand is MN-major (transposed).  acc = 0 overwrites d.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n64(float (&d)[32], uint64_t da, uint64_t db, uint32_t acc) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %34, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, %35, %36;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
 }
+
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_n128(float (&d)[64], uint64_t da, uint64_t db, uint32_t acc) {
+  asm volatile(
+      "{\n"
+      ".reg .pred p;\n"
+      "setp.ne.b32 p, %66, 0;\n"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, %67, %68;\n"
+      "}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(acc), "n"(TA), "n"(TB));
+}
+
+// N = 64 or 128, operand majorness chosen at run time
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t acc, bool a_mn, bool b_mn) {
+  if constexpr (N == 64) {
+    if (a_mn) {
+      if (b_mn) wgmma_n64<1, 1>(d, da, db, acc); else wgmma_n64<1, 0>(d, da, db, acc);
+    } else {
+      if (b_mn) wgmma_n64<0, 1>(d, da, db, acc); else wgmma_n64<0, 0>(d, da, db, acc);
+    }
+  } else {
+    if (a_mn) {
+      if (b_mn) wgmma_n128<1, 1>(d, da, db, acc); else wgmma_n128<1, 0>(d, da, db, acc);
+    } else {
+      if (b_mn) wgmma_n128<0, 1>(d, da, db, acc); else wgmma_n128<0, 0>(d, da, db, acc);
+    }
+  }
+}
+
+// Accumulator fragment of m64nN for thread t of the warpgroup: d[4j + 2h + e] holds row 16*(t/32) + (t%32)/4 + 8h,
+// column 8j + 2*(t%4) + e.
+__device__ __forceinline__ int frag_row(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }
+__device__ __forceinline__ int frag_col(int t) { return (t & 3) << 1; }
 
 }  // namespace bbtc

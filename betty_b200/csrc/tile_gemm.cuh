@@ -9,13 +9,15 @@
 // path lives in gemm_tc.cu.
 #pragma once
 #include "bb_common.cuh"
+#include "plan.h"
 
 namespace bb {
 
 template <int BM, int BN, int BK, int TM, int TN, class LA, class LB, class SC>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 tile_gemm_kernel(const __grid_constant__ LA la, const __grid_constant__ LB lb, const __grid_constant__ SC sc,
-                 int64_t M, int64_t N, int64_t K, int npairs, int ksplit) {
+                 int64_t M, int64_t N, int64_t K, int npairs, int ksplit,
+                 float* __restrict__ part = nullptr) {
   constexpr int THREADS = (BM / TM) * (BN / TN);
   __shared__ float As[BK][BM + 4];
   __shared__ float Bs[BK][BN + 4];
@@ -74,7 +76,9 @@ tile_gemm_kernel(const __grid_constant__ LA la, const __grid_constant__ LB lb, c
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
       const int64_t gn = n0 + tx * TN + j;
-      if (gn < N) sc.store(bz, gm, gn, acc[i][j], split == 0, ksplit > 1);
+      if (gn >= N) continue;
+      if (part != nullptr) part[(((int64_t)split * (gridDim.z / ksplit) + bz) * M + gm) * N + gn] = acc[i][j];
+      else sc.store(bz, gm, gn, acc[i][j], split == 0, ksplit > 1);
     }
   }
 }
@@ -93,7 +97,8 @@ struct VecOperands {
 template <int BM, int BN, int TM, int TN, bool AK, bool BKF, class SC>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 tile_gemm_vec_kernel(const __grid_constant__ VecOperands op, const __grid_constant__ SC sc, int64_t M, int64_t N,
-                     int64_t K, int npairs, int ksplit) {
+                     int64_t K, int npairs, int ksplit,
+                     float* __restrict__ part = nullptr) {
   constexpr int BK = 16;
   constexpr int THREADS = (BM / TM) * (BN / TN);
   __shared__ __align__(16) float As[BK][BM + 4];
@@ -171,7 +176,9 @@ tile_gemm_vec_kernel(const __grid_constant__ VecOperands op, const __grid_consta
 #pragma unroll
     for (int j = 0; j < TN; ++j) {
       const int64_t gn = n0 + tx * TN + j;
-      if (gn < N) sc.store(0, gm, gn, acc[i][j], split == 0, ksplit > 1);
+      if (gn >= N) continue;
+      if (part != nullptr) part[((int64_t)split * M + gm) * N + gn] = acc[i][j];
+      else sc.store(0, gm, gn, acc[i][j], split == 0, ksplit > 1);
     }
   }
 }
@@ -186,6 +193,31 @@ struct StridedLoad {
     return ldf(p[pair], b * bs[pair] + r * rs[pair] + c * cs[pair], dt[pair]);
   }
 };
+
+// Split-K partials part[split][b][m][n] (written by the kernels above when `part` is set) summed in split order, then
+// stored through the caller's store once (bias, beta): the result does not depend on the order the CTAs ran in.
+template <class SC>
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(SC sc, const float* __restrict__ part, int64_t M, int64_t N,
+                                                            int64_t batch, int ksplit) {
+  const int64_t mn = M * N, total = mn * batch;
+  for (int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; t < total; t += (int64_t)gridDim.x * blockDim.x) {
+    float v = 0.f;
+    for (int sp = 0; sp < ksplit; ++sp) v += part[sp * total + t];
+    const int64_t b = t / mn, r = t - b * mn, m = r / N;
+    sc.store(b, m, r - m * N, v, true, false);
+  }
+}
+
+template <class SC>
+inline int splitk_reduce(const SC& sc, const float* part, int64_t M, int64_t N, int64_t batch, int ksplit, cudaStream_t s) {
+  if (part == nullptr || ksplit <= 1) return 0;
+  int64_t blocks = (M * N * batch + 255) / 256;
+  if (blocks > 4096) blocks = 4096;
+  splitk_reduce_kernel<SC><<<(unsigned)blocks, 256, 0, s>>>(sc, part, M, N, batch, ksplit);
+  bb_launch_tally += 1;
+  const cudaError_t e = cudaPeekAtLastError();
+  return e == cudaSuccess ? 0 : (int)e;
+}
 
 struct StridedStore {
   float* p;

@@ -28,6 +28,29 @@ inline void* bb_scratch_alloc(size_t bytes) {
   return bb_scratch.base + at;
 }
 
+// Workspace of the fixed-order reductions (split-K partial products, per-CTA weight-gradient partials): the launcher
+// writes partial sums here and a second kernel adds them in a fixed order, so results do not depend on which CTA
+// finishes first (fp32 atomics would).  Owned by the plan (plan.cu) and published for the duration of its passes; empty
+// outside a plan, where launchers fall back to unsplit reductions.
+struct BbReduceWs {
+  float* base;
+  size_t bytes;
+};
+extern thread_local BbReduceWs bb_reduce_ws;
+inline float* bb_reduce_ws_get(size_t bytes) { return bytes <= bb_reduce_ws.bytes ? bb_reduce_ws.base : nullptr; }
+// Largest split count <= want whose partials (`per_split` bytes each) fit the workspace (1: no split).
+inline int bb_reduce_ws_splits(int want, size_t per_split) {
+  const size_t fit = per_split ? bb_reduce_ws.bytes / per_split : 0;
+  return want <= 1 || fit < 2 ? 1 : (int)(fit < (size_t)want ? fit : (size_t)want);
+}
+
+// out[i] += sum_{b < parts} part[b*n + i], b in order (the second half of a fixed-order reduction; conv_halo.cu)
+int bb_partials_reduce(const float* part, int parts, int64_t n, float* out, cudaStream_t s);
+// A partial buffer of `bytes` for launcher-side reductions: the plan's workspace when it is large enough, otherwise a
+// stream-ordered allocation released by bb_partials_release (launches outside a plan, e.g. the C-ABI unit hooks).
+float* bb_partials_acquire(size_t bytes, cudaStream_t s, bool* owned);
+void bb_partials_release(float* p, bool owned, cudaStream_t s);
+
 // Per-node buffer that lives as long as the plan, for packs of operands that are constant across the K-loop (the
 // im2col matrix of a data-input convolution).  Returns nullptr when the plan has no persistent arena (or it is full);
 // *fresh = true means the caller has to fill it.  Filled eagerly in the base-backward pass (plan creation), so the

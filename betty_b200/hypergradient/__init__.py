@@ -34,7 +34,7 @@ def get_grads(loss, path, retain_graph, do_sync):
 
 
 def install(reference_module=None, callers: bool = False):
-    """Rebind ``betty.hypergradient.jvp_fn_mapping`` entries to the B200 engine.  Returns the table.
+    """Rebind ``betty.hypergradient.jvp_fn_mapping`` entries to the native engine.  Returns the table.
     ``callers=True`` also rebinds the three caller-side methods of SURVEY.md §8 f4 (``betty_b200.callers``:
     flat ``Problem.synchronize_params``, arena ``ImplicitProblem.cache_states`` / ``recover_states``)."""
     if reference_module is None:

@@ -359,7 +359,7 @@ class HvpPlan:
             raise UnsupportedGraph("full reduction of a non-dense tensor")
         r["n"] = xb.numel()
         r["f"][0] = n.attrs["scale"]
-        r["aux"][0] = self._scratch(8 * (2 * 148 + 2)).data_ptr()
+        r["aux"][0] = self._scratch(8 * (2 * 132 + 2)).data_ptr()   # kRedMaxGrid = 2 x BB_SM_COUNT partials
         self._slot(r, 0, x, x.base)
         self._slot(r, 3, n.out, None)
 

@@ -43,9 +43,8 @@ class Tape:
 
 
 # ---- native prologue pieces (SURVEY.md 8 f2) ------------------------------------------------------------------------
-# Training-mode BatchNorm forward on a large channels-first CUDA activation: PyTorch launches one block per channel
-# (5.4 ms for 800 x 64 x 84 x 84 bf16, profiles/r02_launches_maml_final.csv); csrc/bn_fwd.cu does it in 0.4 ms and the
-# whole call gets 7.4 ms (10 %) shorter (profiles/r02_prologue_bn.md).  OPT-IN (BB200_PROLOGUE_BN_MIN=<numel>), off by
+# Training-mode BatchNorm forward on a large channels-first CUDA activation: PyTorch launches one block per channel;
+# csrc/bn_fwd.cu spreads each channel over many blocks and makes the prologue shorter.  OPT-IN (BB200_PROLOGUE_BN_MIN=<numel>), off by
 # default: its statistics differ from aten's in the last fp32 bits, 7e-5 of the bf16 outputs round the other way, and
 # a bf16 4-conv net amplifies that (max-pool / ReLU switches, small-batch statistics) to a 2e-2 ... 6e-2 change of
 # the hypergradient -- inside the reference's own bf16-vs-fp64 gap, but outside the 1e-2 engine-vs-reference bar,

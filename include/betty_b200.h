@@ -1,4 +1,4 @@
-/* betty_b200 -- C ABI of the B200-native hypergradient engine.
+/* betty_b200 -- C ABI of the H100-native hypergradient engine.
  *
  * The reference (leopard-ai/betty) has NO native layer and no FFI: its extension point for this path
  * is the Python plugin table `jvp_fn_mapping[Config.type](vector, curr, prev, sync)`
@@ -85,7 +85,7 @@ int bb_mt_adam_precondition(const bb_mt_adam_chunk* table_dev, int nchunks, void
 /* ---- prologue (SURVEY.md 8 f2): training-mode BatchNorm forward of the lower problem's own forward pass.
  *      Replaces the aten.native_batch_norm(training=True) call PyTorch makes inside curr.training_step_exec
  *      (reference neumann.py:31 / cg.py:27 run that forward once per call) for large channels-first CUDA
- *      activations -- opt-in, BB200_PROLOGUE_BN_MIN (profiles/r02_prologue_bn.md): x, y [N][C][HW] (dtype BB_F32 | BB_BF16), weight / bias fp32 [C] or NULL,
+ *      activations -- opt-in, BB200_PROLOGUE_BN_MIN (betty_b200/trace.py): x, y [N][C][HW] (dtype BB_F32 | BB_BF16), weight / bias fp32 [C] or NULL,
  *      mean / invstd / var_unbiased fp32 [C] (var_unbiased may be NULL), ws >= 2 * C * bb_bn_forward_splits(N, C)
  *      doubles.  out = weight * (x - mean) * invstd + bias, invstd = rsqrt(biased variance + eps); the statistics
  *      are reduced in fp64 in a fixed order.  csrc/bn_fwd.cu                                                  */
@@ -152,7 +152,7 @@ int bb_plan_cg_loop(bb_plan* plan, int iterations, float cg_alpha, float* x, flo
                     const float* hp, int64_t n, void* ws, int use_graph, void* stream);
 
 /* ---- K5 tensor-core building block, exposed for unit tests: C (beta)= A.B with operands rounded to bf16,
- *      fp32 accumulation in TMEM (tcgen05.mma).  A[m][k] = A[m*ars+k*acs], B[k][n] = B[k*brs+n*bcs]; dt: 0 f32, 1 bf16 */
+ *      fp32 accumulation in registers (wgmma.mma_async).  A[m][k] = A[m*ars+k*acs], B[k][n] = B[k*brs+n*bcs]; dt: 0 f32, 1 bf16 */
 int bb_gemm_bf16_tc(int64_t M, int64_t N, int64_t K, const void* A, int dtA, int64_t ars, int64_t acs, const void* B,
                     int dtB, int64_t brs, int64_t bcs, float* C, int64_t crs, int64_t ccs, int beta, void* stream);
 

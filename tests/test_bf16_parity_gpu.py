@@ -3,8 +3,7 @@ backward) run UNDER THE SAME AUTOCAST ON THE SAME GPU (autocast scope = referenc
 neumann.py:59-66 / cg.py:34-56).  BASELINE.json north_star: rtol 1e-2 bf16.
 
 Protocol (SURVEY.md 8c): rel-L2 and allclose(rtol, atol = rtol |ref|_inf) at rtol = 1e-2, with the reference's own
-gap to the float64 evaluation of the same problem measured next to it as the noise floor.  Measured on a B200
-(profiles/r02_bf16_parity.md): the reference's *own* bf16 hypergradient sits 2e-2 ... 2.5e-1 away from float64 on
+gap to the float64 evaluation of the same problem measured next to it as the noise floor.  The reference's *own* bf16 hypergradient sits 2e-2 ... 2.5e-1 away from float64 on
 almost every problem of these shapes (the upper network and the mixed second derivative run in bf16 too; K recurrences
 amplify it) and is pure noise for CG on transformer blocks (4 ... 19 x the answer).  Engine and reference share the
 bf16 forward, so they agree with EACH OTHER far better than either agrees with float64 (6e-3 ... 4e-2 outside CG),

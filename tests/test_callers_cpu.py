@@ -4,6 +4,7 @@
 import copy
 import os
 import socket
+import sys
 import types
 
 import pytest
@@ -162,21 +163,21 @@ def test_arena_snapshot_on_cuda(warm_steps):
     _roll_back_case("cuda", warm_steps, "adam")
 
 
-def test_install_callers_rebinds_reference_methods():
+def test_install_callers_rebinds_reference_methods(monkeypatch):
+    """The reference's layout (betty/problems/problem.py: Problem.synchronize_params; betty/problems/implicit_problem.py:
+    ImplicitProblem.cache_states / recover_states), stood in by empty modules of the same names."""
     from betty_b200 import callers
-    from oracle import reference as R
 
-    if not R.available():
-        pytest.skip("oracle/_ref not mirrored")
-    betty = R.load()
-    from betty.problems.implicit_problem import ImplicitProblem
-    from betty.problems.problem import Problem
-
-    saved = (Problem.synchronize_params, ImplicitProblem.cache_states, ImplicitProblem.recover_states)
-    try:
-        callers.install_callers(betty)
-        assert Problem.synchronize_params is callers.synchronize_params
-        assert ImplicitProblem.cache_states is callers.cache_states
-        assert ImplicitProblem.recover_states is callers.recover_states
-    finally:
-        Problem.synchronize_params, ImplicitProblem.cache_states, ImplicitProblem.recover_states = saved
+    Problem = type("Problem", (), {"synchronize_params": lambda self, params, all_reduce=False: None})
+    ImplicitProblem = type("ImplicitProblem", (Problem,), {"cache_states": lambda self: None,
+                                                            "recover_states": lambda self: None})
+    pkg = types.ModuleType("betty_standin")
+    mods = {"betty_standin": pkg, "betty_standin.problems": types.ModuleType("betty_standin.problems"),
+            "betty_standin.problems.problem": types.SimpleNamespace(Problem=Problem),
+            "betty_standin.problems.implicit_problem": types.SimpleNamespace(ImplicitProblem=ImplicitProblem)}
+    for name, mod in mods.items():
+        monkeypatch.setitem(sys.modules, name, mod)
+    callers.install_callers(pkg)
+    assert Problem.synchronize_params is callers.synchronize_params
+    assert ImplicitProblem.cache_states is callers.cache_states
+    assert ImplicitProblem.recover_states is callers.recover_states

@@ -1,5 +1,5 @@
-"""Unit test of the halo-resident tcgen05 convolution (csrc/conv_halo.cu) through the C ABI: one TMA band of
-128 + 2(W+2) + 2 padded pixel rows per tile, nine taps = nine UMMA descriptors at 128-byte row offsets inside it.
+"""Unit test of the halo-resident wgmma convolution (csrc/conv_halo.cu) through the C ABI: one TMA band of
+128 + 2(W+2) + 2 padded pixel rows per tile, nine taps = nine wgmma descriptors at 128-byte row offsets inside it.
 Operands hold bf16 values, so the only error against the float64 convolution is fp32 accumulation order (2e-5)."""
 import pytest
 import torch

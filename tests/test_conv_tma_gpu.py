@@ -1,4 +1,4 @@
-"""Unit test of the TMA-fed tcgen05 convolution kernels (csrc/conv_tma.cu: `gemm_tma_kernel` with TMA_CONV operands
+"""Unit test of the TMA-fed wgmma convolution kernels (csrc/conv_tma.cu: `gemm_tma_kernel` with TMA_CONV operands
 for the forward / input-gradient products, `wgrad_tma_kernel` for the weight gradient, the im2col route of
 data-input layers) through the C ABI, in the style of test_gemm_tma_gpu.py: a ONE-node plan is built by hand, every
 operand holds bf16-representable values (so the kernels' bf16 operand packs are exact), and each output is compared

@@ -1,4 +1,4 @@
-"""GPU unit test of the tcgen05 tensor-core GEMM building block (csrc/gemm_tc.cu) through the C ABI.
+"""GPU unit test of the wgmma tensor-core GEMM building block (csrc/gemm_tc.cu) through the C ABI.
 Reference = torch matmul of the bf16-rounded operands accumulated in fp32/fp64."""
 import pytest
 import torch

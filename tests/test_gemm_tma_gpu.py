@@ -1,4 +1,4 @@
-"""GPU unit test of the TMA-fed tcgen05 GEMM (csrc/gemm_tma.cu) through the C ABI: every operand layout (k-fast /
+"""GPU unit test of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu) through the C ABI: every operand layout (k-fast /
 m,n-fast storage, fp32 -> packed or bf16 -> direct tensor maps), ragged edges, split-K, beta.
 Reference = matmul of the bf16-rounded operands in fp64."""
 import pytest

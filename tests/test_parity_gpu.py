@@ -1,6 +1,7 @@
 """GPU parity: engine plugins vs (i) the oracle port run on the same device and (ii) the golden vectors
 the real reference produced on CPU (tests/golden, made by oracle/make_golden.py).
 Tolerance: rtol 1e-4 fp32 (BASELINE.json north_star), protocol of SURVEY.md §8(c)."""
+import contextlib
 import glob
 import os
 
@@ -63,7 +64,7 @@ def _tolerance(rec, case):
     of its fp64 value there; those cases use max(1e-4, 5 x that gap)."""
     floor = _reference_floor(rec, case)
     if rec["method"] in ("neumann", "cg"):
-        # 1e-4 hard.  One measured exception (tools/parity_vs_fp64.py, profiles/r02_parity_noise.md): where the REFERENCE's
+        # 1e-4 hard.  One measured exception (tools/parity_vs_fp64.py): where the REFERENCE's
         # own fp32 result on this GPU is not reproducible to 2e-5 (lenet_cg: the conjugate-gradient steps amplify the
         # atomics-order noise of cuDNN's backward to 3e-6 ... 1.3e-4 of the fp64 value, run to run; the engine's own
         # atomics give it the same spread), two fp32 runs -- reference/reference as much as engine/reference -- can only
@@ -78,11 +79,31 @@ def _tolerance(rec, case):
     return tol
 
 
+@contextlib.contextmanager
+def _torch_side_reproducible(hvp_mode):
+    """The test-only autograd hybrid takes its products from torch's double backward, so cuDNN is held to its
+    deterministic algorithms there, for the engine and for the same-device oracle alike.  Otherwise every run of either
+    side is a fresh sample of cuDNN's atomics-order noise (lenet_cg: up to ~1.7e-4 from fp64, against 6e-7 with the
+    deterministic algorithms), which a bar of 1e-4 + the reference's sampled floor does not bound.  The floor itself is
+    still measured with cuDNN's default algorithms."""
+    det = torch.backends.cudnn.deterministic
+    torch.backends.cudnn.deterministic = det or hvp_mode == "autograd"
+    try:
+        yield
+    finally:
+        torch.backends.cudnn.deterministic = det
+
+
+def _engine(rec, wl, hvp_mode):
+    with _torch_side_reproducible(hvp_mode):
+        return H.jvp_fn_mapping[rec["method"]](wl.vector, wl.lower, wl.upper, False)
+
+
 @pytest.mark.parametrize("case", CASES)
 def test_engine_matches_reference_golden(case, hvp_mode):
     rec = load_golden(case)
     wl = W.FACTORIES[rec["factory"]](device="cuda", **rec["kwargs"])
-    got = H.jvp_fn_mapping[rec["method"]](wl.vector, wl.lower, wl.upper, False)
+    got = _engine(rec, wl, hvp_mode)
     assert_close(got, rec["hypergrad"], _tolerance(rec, case), f"{case}[{hvp_mode}]")
 
 
@@ -90,9 +111,10 @@ def test_engine_matches_reference_golden(case, hvp_mode):
 def test_engine_matches_oracle_same_device(case, hvp_mode):
     rec = load_golden(case)
     wl = W.FACTORIES[rec["factory"]](device="cuda", **rec["kwargs"])
-    want = ref_port.METHODS[rec["method"]](wl.vector, wl.lower, wl.upper, False)
+    with _torch_side_reproducible(hvp_mode):
+        want = ref_port.METHODS[rec["method"]](wl.vector, wl.lower, wl.upper, False)
     w_before = [p.detach().clone() for p in wl.lower.parameters()]
-    got = H.jvp_fn_mapping[rec["method"]](wl.vector, wl.lower, wl.upper, False)
+    got = _engine(rec, wl, hvp_mode)
     tol = _tolerance(rec, case)
     if hvp_mode == "autograd":
         # test-only hybrid (products by torch autograd): BOTH sides are then fp32 runs with atomics in cuDNN / index_add,

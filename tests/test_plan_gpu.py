@@ -28,7 +28,7 @@ CASES = {
     "roberta": ("bert_data_reweighting", dict(batch=3, seq=9, tiny=True), 2e-5),
     "fourconv_bf16": ("implicit_maml", dict(n=10, hidden=16, precision="bf16"), 3e-2),
     "roberta_bf16": ("bert_data_reweighting", dict(batch=3, seq=9, tiny=True, precision="bf16"), 3e-2),
-    # 128 tokens x hidden 128: the Linear products are large enough for the tcgen05 tensor-core kernel
+    # 128 tokens x hidden 128: the Linear products are large enough for the wgmma tensor-core kernel
     "roberta_bf16_tc": ("bert_data_reweighting", dict(batch=8, seq=16, tiny=True, tiny_hidden=128, precision="bf16"), 4e-2),
     # 64-channel 3x3 convolutions on the tensor-core implicit-GEMM path (forward / data-grad / weight-grad gathers)
     # 40 tokens x head_dim 64: the batched attention products go through the TMA-fed tensor-core kernel as well

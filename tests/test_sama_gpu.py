@@ -1,21 +1,24 @@
-"""``sama`` (SURVEY.md 8 f3): the B200 plugin against the REAL reference function ``betty.hypergradient.sama.sama``
-(oracle/_ref) on the same GPU, with a lower Adam optimizer whose state carries exp_avg / exp_avg_sq / last_grad the way
-the reference's ImplicitProblem stores them (implicit_problem.py:50-66), and with SGD (identity preconditioner)."""
-import importlib
+"""``sama`` (SURVEY.md 8 f3): the plugin against what the REAL reference function ``betty.hypergradient.sama.sama``
+returns on the same seeded inputs (tests/golden/sama, made by oracle/make_golden.py), with a lower Adam optimizer whose
+state carries exp_avg / exp_avg_sq / last_grad the way the reference's ImplicitProblem stores them
+(implicit_problem.py:50-66), and with SGD (identity preconditioner)."""
+import os
 
 import pytest
 import torch
 
 from betty_b200 import hypergradient as H
-from betty_b200 import workloads as W
-from oracle import reference as R
+from oracle import make_golden as MG
 from tests.helpers import assert_close, rel_l2
 
-pytestmark = [pytest.mark.gpu, pytest.mark.skipif(not R.available(), reason="oracle/_ref not fetched")]
+pytestmark = pytest.mark.gpu
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "sama")
 
 
-def _adam_state(wl, steps=3, lr=1e-2):
-    return W.attach_adam_state(wl, steps, lr).lower.optimizer
+def _golden(name, wl):
+    rec = torch.load(os.path.join(GOLDEN, name + ".pt"), weights_only=False)
+    assert abs(MG.input_checksum(wl) - rec["checksum"]) <= 1e-6 * max(1.0, abs(rec["checksum"])), "inputs drifted"
+    return rec
 
 
 @pytest.mark.parametrize("case", ["logistic", "mlp", "lenet"])
@@ -23,17 +26,11 @@ def _adam_state(wl, steps=3, lr=1e-2):
 def test_sama_matches_the_reference_function(case, optimizer):
     torch.backends.cudnn.allow_tf32 = False
     torch.backends.cuda.matmul.allow_tf32 = False
-    R.load()
-    ref_sama = importlib.import_module("betty.hypergradient.sama").sama
-    fac, kw = {"logistic": ("logistic_regression_hpo", dict(method="sama")),
-               "mlp": ("mlp_reweight", dict(method="sama")),
-               "lenet": ("learning_to_reweight", dict(method="sama", batch=32))}[case]
-    wl = W.FACTORIES[fac](device="cuda", **kw)
-    wl.lower.config.sama_adam_alpha = 1.0
-    if optimizer == "sgd":      # (the factories attach an Adam state for method="sama")
-        wl.lower.optimizer = torch.optim.SGD(wl.lower.module.parameters(), lr=0.1)
+    name = f"sama_{optimizer}_{case}"
+    fac, kw, opt = MG.SAMA_CASES[name]
+    wl = MG.sama_workload(fac, kw, opt, device="cuda")     # seeded on the CPU generator, as the golden run was
+    want = [t.cuda() for t in _golden(name, wl)["hypergrad"]]
     w_before = [p.detach().clone() for p in wl.lower.parameters()]
-    want = ref_sama(wl.vector, wl.lower, wl.upper, False)
     got = H.sama(wl.vector, wl.lower, wl.upper, False)
     # finite differences in fp32: the reference's own noise floor applies (SURVEY 8c); measured against float64 below
     assert_close(got, want, 5e-3 if case != "logistic" else 1e-3, f"sama {case}/{optimizer}")
@@ -49,14 +46,11 @@ def test_sama_matches_the_reference_function(case, optimizer):
 def test_adam_preconditioner_kernel_against_the_reference_formula():
     from betty_b200.hypergradient.sama import precondition
 
-    R.load()
-    ref_pre = importlib.import_module("betty.hypergradient.utils").precondition
-    wl = W.mlp_reweight(device="cuda", method="sama")
-    wl.lower.optimizer = _adam_state(wl, steps=4)
-    want = ref_pre(list(wl.vector), wl.lower)
+    wl = MG.precondition_workload(device="cuda")
+    rec = _golden("precondition", wl)
     got = precondition(list(wl.vector), wl.lower)
-    assert_close(got, want, 1e-5, "adam preconditioner")
+    assert_close(got, [t.cuda() for t in rec["adam"]], 1e-5, "adam preconditioner")
     # a parameter without state (never stepped): the reference substitutes zeros, so does the kernel
     p0 = next(iter(wl.lower.module.parameters()))
     wl.lower.optimizer.state[p0] = {}
-    assert_close(precondition(list(wl.vector), wl.lower), ref_pre(list(wl.vector), wl.lower), 1e-5, "empty state")
+    assert_close(precondition(list(wl.vector), wl.lower), [t.cuda() for t in rec["adam_empty_first"]], 1e-5, "empty state")

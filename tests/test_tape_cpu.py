@@ -309,7 +309,7 @@ def test_side_computations_without_a_rule_do_not_abort():
 
 def test_native_prologue_batchnorm_is_opt_in_and_never_touches_cpu_tensors(monkeypatch):
     """The recorder substitutes aten.native_batch_norm only when asked to (BB200_PROLOGUE_BN_MIN) and only for CUDA
-    inputs (betty_b200/trace.py, profiles/r02_prologue_bn.md): by default the lower forward is PyTorch's, bit for bit."""
+    inputs (betty_b200/trace.py): by default the lower forward is PyTorch's, bit for bit."""
     import torch
 
     from betty_b200 import trace as T

@@ -1,35 +1,14 @@
 """The synthetic workloads restate the reference examples' models (betty_b200/workloads.py cites each); this pins the
-config-4 restatement -- Network(16, 10, 8) + Architecture(4) -- to the reference's own classes (mirrored under
-oracle/_ref by oracle/fetch_ref.sh): identical parameter list and identical logits on the same weights."""
-import importlib
+config-4 restatement -- Network(16, 10, 8) + Architecture(4) -- to the reference's own classes: identical parameter list
+and identical logits on the same weights (tests/golden/models/darts_network.pt, made by oracle/make_golden.py from the
+reference's examples/neural_architecture_search/model_search.py)."""
 import os
-import sys
-import types
 
-import pytest
 import torch
 
 from betty_b200 import workloads as W
-from oracle import reference as R
 
-NAS_DIR = os.path.join(R.REF_ROOT, "examples", "neural_architecture_search")
-
-
-def _reference_model_search():
-    saved = {k: sys.modules.get(k) for k in ("utils", "operations", "genotypes", "model_search")}
-    sys.modules["utils"] = types.SimpleNamespace(accuracy=None)     # model_search imports it for an unused helper
-    sys.path.insert(0, NAS_DIR)
-    try:
-        for k in ("operations", "genotypes", "model_search"):
-            sys.modules.pop(k, None)
-        return importlib.import_module("model_search")
-    finally:
-        sys.path.remove(NAS_DIR)
-        for k, v in saved.items():
-            if v is None:
-                sys.modules.pop(k, None)
-            else:
-                sys.modules[k] = v
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "models", "darts_network.pt")
 
 
 def test_full_size_darts_network_has_the_survey_sizes():
@@ -39,19 +18,12 @@ def test_full_size_darts_network_has_the_survey_sizes():
     assert sum(p.numel() for p in arch.parameters()) == 2 * 14 * 8
 
 
-@pytest.mark.skipif(not os.path.isdir(NAS_DIR), reason="oracle/_ref not fetched")
 def test_full_size_darts_network_matches_the_reference_classes():
-    MS = _reference_model_search()
+    rec = torch.load(GOLDEN, weights_only=False)
     torch.manual_seed(0)
-    ref, ref_arch = MS.Network(16, 10, 8, None), MS.Architecture(4)
     net, arch = W.DartsSearchNetwork(16, 10, 8), W.DartsArchitecture(4)
-    mine, theirs = list(net.parameters()), list(ref.parameters())
-    assert [tuple(p.shape) for p in mine] == [tuple(p.shape) for p in theirs]
+    assert [tuple(p.shape) for p in net.parameters()] == [tuple(s) for s in rec["shapes"]]
+    x = torch.randn(2, 3, 32, 32, generator=torch.Generator().manual_seed(1))
+    net.train()
     with torch.no_grad():
-        for a, b in zip(mine, theirs):
-            a.copy_(b)
-        for a, b in zip(arch.parameters(), ref_arch.parameters()):
-            a.copy_(b)
-    x = torch.randn(2, 3, 32, 32)
-    net.train(), ref.train()
-    assert torch.allclose(net(x, arch()), ref(x, ref_arch()), rtol=1e-5, atol=1e-6)
+        assert torch.allclose(net(x, arch()), rec["logits"], rtol=1e-5, atol=1e-6)

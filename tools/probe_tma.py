@@ -1,4 +1,4 @@
-"""GPU probe of the TMA-fed tcgen05 GEMM (csrc/gemm_tma.cu): error vs a bf16-rounded fp64 matmul for every operand
+"""GPU probe of the TMA-fed wgmma GEMM (csrc/gemm_tma.cu): error vs a bf16-rounded fp64 matmul for every operand
 layout, then throughput on large shapes next to the software-staged kernel.  Usage: python tools/probe_tma.py"""
 import sys
 import os

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel SASS mnemonic counts of the built library: the committed evidence that the tensor-core kernels are
-Blackwell-native (UTCHMMA = tcgen05.mma, UTMALDG = TMA loads, LDTM = tcgen05.ld, UTCBAR = tcgen05.commit) and which
-kernels run on the legacy warp-level path (HMMA = mma.sync).  Usage: python tools/sass_summary.py > profiles/rNN_sass.txt"""
+Hopper-native (HGMMA = wgmma.mma_async, UTMALDG = TMA loads, WARPGROUP = wgmma fences / waits) and which kernels run on
+the legacy warp-level path (HMMA = mma.sync).  Usage: python tools/sass_summary.py > sass.txt"""
 import collections
 import os
 import re
@@ -10,7 +10,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SO = os.path.join(ROOT, "betty_b200", "csrc", "libbetty_b200.so")
-WATCH = ["UTCHMMA", "UTCQMMA", "UTCBAR", "UTMALDG", "UTMASTG", "UTMAPF", "LDTM", "STTM", "UTCATOM", "HMMA", "LDSM",
+WATCH = ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "UTMAPF", "HMMA", "LDSM",
          "SYNCS", "FFMA", "LDG", "STG", "LDS", "STS", "ATOM", "RED", "ELECT"]
 
 
@@ -35,12 +35,12 @@ def main():
                 if op.startswith(w):
                     cur[w] += 1
                     break
-    print(f"# cuobjdump -sass betty_b200/csrc/libbetty_b200.so  ({ver}; -gencode arch=compute_100a,code=sm_100a)")
-    print("# UTCHMMA = tcgen05.mma (kind::f16), UTMALDG = cp.async.bulk.tensor (TMA), LDTM = tcgen05.ld, "
-          "UTCBAR = tcgen05.commit, HMMA = mma.sync (legacy warp-level path), LDSM = ldmatrix")
-    tc = [(k, c) for k, c in counts.items() if c["UTCHMMA"] or c["UTMALDG"] or c["LDTM"]]
-    hm = [(k, c) for k, c in counts.items() if c["HMMA"] and not c["UTCHMMA"]]
-    rest = [(k, c) for k, c in counts.items() if not (c["UTCHMMA"] or c["UTMALDG"] or c["LDTM"] or c["HMMA"])]
+    print(f"# cuobjdump -sass betty_b200/csrc/libbetty_b200.so  ({ver}; -gencode arch=compute_90a,code=sm_90a)")
+    print("# HGMMA = wgmma.mma_async, WARPGROUP = wgmma.fence / wait_group, UTMALDG = cp.async.bulk.tensor (TMA), "
+          "HMMA = mma.sync (legacy warp-level path), LDSM = ldmatrix")
+    tc = [(k, c) for k, c in counts.items() if c["HGMMA"] or c["UTMALDG"]]
+    hm = [(k, c) for k, c in counts.items() if c["HMMA"] and not c["HGMMA"]]
+    rest = [(k, c) for k, c in counts.items() if not (c["HGMMA"] or c["UTMALDG"] or c["HMMA"])]
 
     def short(k):
         k = k.replace("(anonymous namespace)::", "").replace("void ", "")
@@ -53,8 +53,8 @@ def main():
         for k, c in sorted(rows, key=lambda kc: kc[0]):
             print(f"| `{short(k)}` | {c['_total']} | " + " | ".join(str(c[w]) for w in cols) + " |")
 
-    print(f"\n## tcgen05 / TMA kernels ({len(tc)})\n")
-    table(tc, ["UTCHMMA", "UTCBAR", "UTMALDG", "UTMASTG", "LDTM", "SYNCS", "ELECT", "HMMA"])
+    print(f"\n## wgmma / TMA kernels ({len(tc)})\n")
+    table(tc, ["HGMMA", "WARPGROUP", "UTMALDG", "UTMASTG", "SYNCS", "ELECT", "HMMA"])
     print(f"\n## warp-level tensor-core kernels, mma.sync ({len(hm)})\n")
     table(hm, ["HMMA", "LDSM", "LDG", "STG", "LDS", "STS", "FFMA"])
     print(f"\n## SIMT kernels ({len(rest)})\n")
