@@ -139,9 +139,15 @@ int launch(const LA& la, const LB& lb, const SC& sc, int64_t M, int64_t N, int64
   return bb::splitk_reduce(sc, part, M, N, 1, ksplit, s);
 }
 
-// out[ch] += sum_{img, q} g[(img*CH + ch)*HW + q]
+__device__ __forceinline__ void chansum_store(float* out, float* part, int ch, int CH, float acc) {
+  if (part != nullptr) part[(int64_t)blockIdx.y * CH + ch] = acc;
+  else out[ch] += acc;
+}
+
+// out[ch] += sum_{img, q} g[(img*CH + ch)*HW + q].  With part != nullptr, block (ch, y) writes its sum to part[y*CH + ch]
+// and bb_partials_reduce adds the gridDim.y partials in order; without, gridDim.y is 1 and the block adds to out itself.
 __global__ void __launch_bounds__(256) chansum_kernel(const float* __restrict__ g, float* out, int NIMG, int CH, int HW,
-                                                      int small_max) {
+                                                      int small_max, float* __restrict__ part) {
   __shared__ float red[32];
   const int ch = blockIdx.x;
   float acc = 0.f;
@@ -171,7 +177,7 @@ __global__ void __launch_bounds__(256) chansum_kernel(const float* __restrict__ 
       acc += (part[0] + part[1]) + (part[2] + part[3]);
     }
     acc = bb::block_sum<float>(acc, red);
-    if (threadIdx.x == 0) atomicAdd(out + ch, acc);
+    if (threadIdx.x == 0) chansum_store(out, part, ch, CH, acc);
     return;
   }
   for (int img = blockIdx.y; img < NIMG; img += gridDim.y) {
@@ -186,7 +192,7 @@ __global__ void __launch_bounds__(256) chansum_kernel(const float* __restrict__ 
     }
   }
   acc = bb::block_sum<float>(acc, red);
-  if (threadIdx.x == 0) atomicAdd(out + ch, acc);
+  if (threadIdx.x == 0) chansum_store(out, part, ch, CH, acc);
 }
 
 // ---- tensor-core (wgmma) implicit-GEMM operands, bf16-autocast graphs with >= 32 channels ----------
@@ -385,10 +391,14 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
       bb_launch_tally += 1;
     }
     int gy_blocks = g.N < 64 ? g.N : 64;
+    gy_blocks = bb_reduce_ws_splits(gy_blocks, sizeof(float) * g.O);     // 1 outside a plan: no partials
+    float* part = gy_blocks > 1 ? bb_reduce_ws.base : nullptr;
     static const int small_max = getenv("BB200_CHANSUM_V1") ? 0 : 512;
-    chansum_kernel<<<dim3(g.O, gy_blocks), 256, 0, s>>>(reinterpret_cast<const float*>(gy), out, g.N, g.O, g.HO * g.WO, small_max);
+    chansum_kernel<<<dim3(g.O, gy_blocks), 256, 0, s>>>(reinterpret_cast<const float*>(gy), out, g.N, g.O, g.HO * g.WO,
+                                                        small_max, part);
     bb_launch_tally += 1;
     BB_LAUNCH_CHECK();
+    if (part != nullptr && (rc = bb_partials_reduce(part, gy_blocks, g.O, out, s))) return rc;
   }
   return BB_OK;
 }

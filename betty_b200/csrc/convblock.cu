@@ -1137,8 +1137,10 @@ int run(const CbArgs& A0, int pass, cudaStream_t s) {
     BB_CUDA_TRY(cudaFuncSetAttribute(cb_prep_kernel<PT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
   }
   if (smem_red > 200 * 1024 || (size_t)g.WP * g.O * 9 > 200 * 1024) return BB_ERR_UNSUPPORTED;
-  // tensor-core path of the K-loop kernels: bf16 pooled arrays, 64 channels, NHWC neighbour on the pooled side
-  static const bool no_mma = getenv("BB200_NO_CBMMA") != nullptr;
+  // tensor-core path of the K-loop kernels: bf16 pooled arrays, 64 channels, NHWC neighbour on the pooled side.
+  // BB200_NO_CBMMA is read at each launch, so a process can run both routes; a plan must keep one route for all passes
+  // (the base pass builds the state its tangent passes read).
+  const bool no_mma = getenv("BB200_NO_CBMMA") != nullptr;
   const bool mma = !no_mma && g.O == 64 && sizeof(PT) == 2 && A.tq_nhwc && A.atq_nhwc && A.w.pfrag;
   const int64_t nmt = ((int64_t)g.N * g.HP * g.WP + MT - 1) / MT;
   auto mma_blocks = [&](const void* fn, size_t smem) {
