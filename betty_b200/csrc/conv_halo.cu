@@ -40,6 +40,7 @@ constexpr int BAND_ROWS = 256;                 // TMA box limit; a band needs 12
 constexpr int BAND_BYTES = BAND_ROWS * 128;    // 32 KB
 constexpr int W_TILE = 64 * 128;               // one tap's weights: 64 rows (n) x 64 ch
 constexpr int MAXBAND = 4;                     // activation bands in flight: 4 with one operand pair, 2 with two
+constexpr int STG_BYTES = 64 * 128;            // one warpgroup's 64 output rows in bf16
 
 struct alignas(64) HaloArgs {
   CUtensorMap a[2];          // padded activation as a matrix [rows][64] (rank-3 map, batch 1), box (64, band_rows)
@@ -62,7 +63,7 @@ struct alignas(64) HaloArgs {
 
 
 // Shared memory: [npairs x 9 x 8 KB] weights (resident for the whole kernel) | [NB x band_alloc] activation bands |
-// barriers.  The MMA issue loop stays free of waits: both pairs' weights are resident rather than streamed through a
+// [2 x 8 KB] bf16 output staging, one 64-row block per consumer warpgroup (BF16OUT only) | barriers.  The MMA issue loop stays free of waits: both pairs' weights are resident rather than streamed through a
 // ring with a wait per tap, and two bands are in flight.
 template <int NB, bool BF16OUT>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_constant__ HaloArgs G) {
@@ -70,7 +71,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* wsm = smem;                                    // [npairs][9][W_TILE]
   uint8_t* bands = smem + (size_t)G.npairs * 9 * W_TILE;  // [NB][band_alloc]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(bands + (size_t)NB * G.band_alloc);
+  uint8_t* stg = bands + (size_t)NB * G.band_alloc;      // [2][64 rows x 128 B]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(stg + (BF16OUT ? 2 * STG_BYTES : 0));
   const uint32_t wfull = smem_u32(bars);
   const uint32_t bfull0 = smem_u32(bars + 1), bempty0 = smem_u32(bars + 1 + MAXBAND);
 
@@ -151,37 +153,56 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
     fence_acc(acc);
     if (t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
     // ---------------- epilogue: d[4j + 2h + e] = (row frag_row + 8h, channel 8j + frag_col + e) ----------------
+    if constexpr (BF16OUT) {
+      // bf16 padded-NHWC output: this warpgroup's 64 rows are one contiguous 8 KB block of the output.  Stored from the
+      // fragments, each warp store would cover eight half sectors; staged in shared memory (16-byte chunk j of row r at
+      // r*128 + 16 (j ^ (r & 7)), free of bank conflicts) it goes out as whole 16-byte chunks, border rows as zeros.
+      uint8_t* st = stg + wg * STG_BYTES;
+      named_barrier_sync(1 + wg, 128);    // per warpgroup; the previous tile's copy-out has read the staging block
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int64_t row = (int64_t)tile * BM + wg * 64 + frag_row(t) + 8 * h;   // padded-linear pixel index
-      if (row >= G.total_rows) continue;
-      const int img = (int)(row / G.HpWp);
-      const int rem = (int)(row - (int64_t)img * G.HpWp);
-      const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
-      const bool ok = yy >= 1 && yy <= G.H && xx >= 1 && xx <= G.W;
-      if (BF16OUT) {
-        // bf16 padded-NHWC output: this pixel row's 64 channels; border rows are zeros
-        __nv_bfloat162* q = reinterpret_cast<__nv_bfloat162*>(G.out_bf16 + row * 64 + frag_col(t));
+      for (int h = 0; h < 2; ++h) {
+        const int r = frag_row(t) + 8 * h;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int n = 8 * j + frag_col(t);
           float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
           if (G.bias) { f0 += G.bias[n]; f1 += G.bias[n + 1]; }
-          q[4 * j] = ok ? __floats2bfloat162_rn(f0, f1) : __floats2bfloat162_rn(0.f, 0.f);
+          *reinterpret_cast<__nv_bfloat162*>(st + r * 128 + 16 * (j ^ (r & 7)) + 2 * frag_col(t)) = __floats2bfloat162_rn(f0, f1);
         }
-        continue;
       }
-      if (!ok) continue;
-      float* q = G.out + (int64_t)img * BN * HW + (int64_t)(yy - 1) * G.W + (xx - 1);
+      named_barrier_sync(1 + wg, 128);
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
+      for (int it = 0; it < 4; ++it) {
+        const int k = t + 128 * it, r = k >> 3, c = k & 7;
+        const int64_t row = (int64_t)tile * BM + wg * 64 + r;   // padded-linear pixel index
+        if (row >= G.total_rows) break;
+        const int img = (int)(row / G.HpWp);
+        const int rem = (int)(row - (int64_t)img * G.HpWp);
+        const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if (yy >= 1 && yy <= G.H && xx >= 1 && xx <= G.W) v = *reinterpret_cast<const uint4*>(st + r * 128 + 16 * (c ^ (r & 7)));
+        *reinterpret_cast<uint4*>(G.out_bf16 + row * 64 + 8 * c) = v;
+      }
+    } else {
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int n = 8 * j + frag_col(t) + e;
-          float v = acc[4 * j + 2 * h + e];
-          if (G.bias) v += G.bias[n];
-          float* d = q + (int64_t)n * HW;
-          *d = G.beta ? *d + v : v;
+      for (int h = 0; h < 2; ++h) {
+        const int64_t row = (int64_t)tile * BM + wg * 64 + frag_row(t) + 8 * h;   // padded-linear pixel index
+        if (row >= G.total_rows) continue;
+        const int img = (int)(row / G.HpWp);
+        const int rem = (int)(row - (int64_t)img * G.HpWp);
+        const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
+        if (yy < 1 || yy > G.H || xx < 1 || xx > G.W) continue;
+        float* q = G.out + (int64_t)img * BN * HW + (int64_t)(yy - 1) * G.W + (xx - 1);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int n = 8 * j + frag_col(t) + e;
+            float v = acc[4 * j + 2 * h + e];
+            if (G.bias) v += G.bias[n];
+            float* d = q + (int64_t)n * HW;
+            *d = G.beta ? *d + v : v;
+          }
         }
       }
     }
@@ -213,6 +234,7 @@ constexpr int WH_G_BYTES = 128 * 128;     // 16 KB
 constexpr int WH_STAGE = BAND_BYTES + WH_G_BYTES;
 constexpr int WH_CONSUMERS = 3;
 constexpr int WH_THREADS = WH_CONSUMERS * 128 + 32;
+static_assert(64 * 64 * 9 * 4 <= 4 * WH_STAGE, "the weight-gradient partial is staged in the four stage buffers");
 
 __global__ void __launch_bounds__(WH_THREADS, 1) wgrad_halo_kernel(const __grid_constant__ WHaloArgs G) {
   extern __shared__ uint8_t smem_raw[];
@@ -289,6 +311,11 @@ __global__ void __launch_bounds__(WH_THREADS, 1) wgrad_halo_kernel(const __grid_
     if (it > 0 && t == 0) mbar_arrive(empty0 + 8 * ((it - 1) % G.stages));
   }
   wgmma_wait<0>();
+  // The CTA's partial [O][C][9] goes out through shared memory: written straight from the fragments, every 4-byte
+  // store would land in its own 32-byte sector (consecutive taps of one (o, c) sit in different warpgroups).  The
+  // stage buffers are idle once every consumer has drained its last wgmma.
+  named_barrier_sync(1, WH_CONSUMERS * 128);
+  float* stage = reinterpret_cast<float*>(smem);
 #pragma unroll
   for (int q = 0; q < 3; ++q) {
     fence_acc(acc[q]);
@@ -303,10 +330,14 @@ __global__ void __launch_bounds__(WH_THREADS, 1) wgrad_halo_kernel(const __grid_
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int o = 8 * j + frag_col(t) + e;
-          if (o < G.O) G.part[((int64_t)blockIdx.x * G.O * G.C + (int64_t)o * G.C + c) * 9 + tap] = acc[q][4 * j + 2 * h + e];
+          if (o < G.O) stage[(o * G.C + c) * 9 + tap] = acc[q][4 * j + 2 * h + e];
         }
     }
   }
+  named_barrier_sync(1, WH_CONSUMERS * 128);
+  const int n = G.O * G.C * 9;
+  float* dst = G.part + (int64_t)blockIdx.x * n;
+  for (int i = tid; i < n; i += WH_CONSUMERS * 128) dst[i] = stage[i];
 }
 
 __global__ void __launch_bounds__(256) partials_reduce_kernel(const float* __restrict__ part, int parts, int64_t n,
@@ -369,14 +400,14 @@ int bb_conv_halo_run(int N, int H, int W, int npairs, const void* const* act_pad
     if ((rc = bb_tma_map_2d(&G.b[p], wmat[p], 64, 9 * 64, 9 * 64, 64))) return rc;
   }
   G.band_alloc = (G.band_rows * 128 + 1023) & ~1023;
-  const size_t fixed = (size_t)npairs * 9 * W_TILE + 512 + 1024;
+  const bool bf = G.out_bf16 != nullptr;
+  const size_t fixed = (size_t)npairs * 9 * W_TILE + (bf ? 2 * STG_BYTES : 0) + 512 + 1024;
   const int fit = (int)((227 * 1024 - fixed) / (size_t)G.band_alloc);
   if (fit < 2) return BB_ERR_UNSUPPORTED;
   const int nb = fit >= 4 ? 4 : 2;
   G.nband = nb;
   const size_t smem = fixed + (size_t)nb * G.band_alloc;
   const int grid = G.ntiles < BB_SM_COUNT ? G.ntiles : BB_SM_COUNT;
-  const bool bf = G.out_bf16 != nullptr;
   static BbOncePerDevice configured[4];
   auto launch = [&](auto kern, int slot) -> int {
     if (configured[slot].need())

@@ -145,6 +145,11 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint6
   }
 }
 
+// barrier among `count` threads (a multiple of 32) on hardware barrier `id` (0 is __syncthreads)
+__device__ __forceinline__ void named_barrier_sync(int id, int count) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
 // Accumulator fragment of m64nN for thread t of the warpgroup: d[4j + 2h + e] holds row 16*(t/32) + (t%32)/4 + 8h,
 // column 8j + 2*(t%4) + e.
 __device__ __forceinline__ int frag_row(int t) { return ((t >> 5) << 4) + ((t & 31) >> 2); }

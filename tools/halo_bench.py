@@ -1,6 +1,8 @@
-"""Time the halo convolution / weight-gradient kernels alone at the implicit-MAML shapes (CUDA events on the launch
-stream, L2 flushed between launches by rotating over operand sets larger than L2).  Environment switches of
-csrc/conv_halo.cu (BB200_HALO_PIECES, BB200_HALO_STREAM_W) are read once per process: run one process per variant.
+"""Time the halo convolution / weight-gradient kernels alone at the three shapes the implicit-MAML benchmark runs them
+(N=800 at 42x42, 21x21 and 10x10; CUDA events on the launch stream, L2 flushed between launches by rotating over
+operand sets larger than L2).  TF/s are given from useful FLOPs (N*H*W pixels) and from padded FLOPs (every 128-row
+tile of the padded layout, which is what the tensor cores execute), with the useful rate as a fraction of the H100
+SXM data-sheet 989 dense BF16 TFLOP/s.  With BB200_LIB=<path> the same run times another build of the library.
     python tools/halo_bench.py [N H W]"""
 import os
 import sys
@@ -10,9 +12,10 @@ import torch
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 from betty_b200 import _native as N
 
+PEAK_TFLOPS = 989.0
 
-def main():
-    n, h, w = (int(a) for a in sys.argv[1:4]) if len(sys.argv) >= 4 else (800, 42, 42)
+
+def bench_shape(n, h, w):
     dev = torch.device("cuda")
     g = torch.Generator(device="cuda").manual_seed(1)
     nset = 3
@@ -23,7 +26,7 @@ def main():
     wg = torch.zeros(64, 64, 3, 3, device=dev)
     st = torch.cuda.current_stream().cuda_stream
 
-    def timed(fn, reps=12):
+    def timed(fn, reps=20):
         for i in range(3):
             fn(i % nset)
         torch.cuda.synchronize()
@@ -49,15 +52,27 @@ def main():
                                 acts[(i + 1) % nset][0].data_ptr(), acts[(i + 1) % nset][1].data_ptr() if np_ > 1 else 0,
                                 wg.data_ptr(), st)
 
-    flops = 2.0 * n * h * w * 64 * 64 * 9
-    env = {k: v for k, v in os.environ.items() if k.startswith("BB200_")}
-    print(f"shape N={n} H={h} W={w} env={env}")
-    runs = [("conv->nchw f32,  1 pair", conv_f32(1), 1), ("conv->nchw f32,  2 pairs", conv_f32(2), 2), ("wgrad, 2 pairs", wgrad(2), 2)]
-    if "BB200_LIB" not in os.environ:
-        runs += [("conv->nhwc bf16, 1 pair", conv_nhwc(1), 1), ("conv->nhwc bf16, 2 pairs", conv_nhwc(2), 2)]
+    per_px = 2.0 * 64 * 64 * 9
+    useful = per_px * n * h * w
+    padded = per_px * -(-n * (h + 2) * (w + 2) // 128) * 128
+    print(f"shape N={n} H={h} W={w}")
+    runs = [("conv->nhwc bf16, 2 pairs", conv_nhwc(2), 2), ("conv->nhwc bf16, 1 pair", conv_nhwc(1), 1),
+            ("conv->nchw f32,  2 pairs", conv_f32(2), 2), ("conv->nchw f32,  1 pair", conv_f32(1), 1),
+            ("wgrad, 2 pairs", wgrad(2), 2)]
     for name, fn, np_ in runs:
         us = timed(fn)
-        print(f"  {name:28s} {us:8.1f} us   {np_ * flops / us * 1e-6:7.1f} TF/s")
+        tf = np_ * useful / us * 1e-6
+        print(f"  {name:26s} {us:8.1f} us   {tf:6.1f} TF/s useful ({tf / PEAK_TFLOPS:5.1%} of {PEAK_TFLOPS:.0f})"
+              f"   {np_ * padded / us * 1e-6:6.1f} TF/s padded")
+    del acts, outp, outf
+    torch.cuda.empty_cache()
+
+
+def main():
+    print(f"device: {torch.cuda.get_device_name()}   library: {os.environ.get('BB200_LIB', N.LIB_PATH)}")
+    shapes = [tuple(int(a) for a in sys.argv[1:4])] if len(sys.argv) >= 4 else [(800, 42, 42), (800, 21, 21), (800, 10, 10)]
+    for n, h, w in shapes:
+        bench_shape(n, h, w)
 
 
 if __name__ == "__main__":
