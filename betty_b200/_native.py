@@ -69,6 +69,8 @@ _SIGS = {
     "bb_plan_node_route": ([C.c_void_p, C.c_int, C.c_int], 0),
     "bb_conv_halo_bf16": ([C.c_int] * 4 + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p], 1),
     "bb_conv_halo_bf16_nhwc": ([C.c_int] * 4 + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p], 1),
+    "bb_conv_halo_phases": ([C.c_int] * 4 + [C.c_void_p] * 4 + [C.c_int] + [C.c_void_p] * 5, None),
+    "bb_conv_halo_phase_names": ([C.c_char_p, C.c_int], 0),
     "bb_wgrad_halo_bf16": ([C.c_int] * 4 + [C.c_void_p] * 6, 1),
     "bb_convblock_ws_bytes": ([C.c_int] * 9, 0),
     "bb_convblock2_ws_bytes": ([C.c_int] * 9, 0),

@@ -59,13 +59,29 @@ struct alignas(64) HaloArgs {
                              // row tile*128 + r of the output matrix: one contiguous 16 KB block per tile), border rows 0
   int beta;
   const float* bias;
+  unsigned long long* phases;   // PHASES variant only: see bb_conv_halo_phases
+  int phase_slots;              // tile slots per CTA in `phases` (tiles per CTA + 1)
 };
+
+// Phase timing (conv_halo_kernel<..., PHASES = true>, reached only through bb_conv_halo_phases): thread 0 of each
+// consumer warpgroup writes clock64() at the points named by PHASE_NAMES, in program order, into
+//   phases[4 * grid + ((cta * phase_slots + slot) * 2 + wg) * NSTAMP + k]
+// and thread 0 of the CTA writes {globaltimer, clock64} at the start and the end of its tile loop into phases[4 * cta ...]
+// (so the SM clock can be recovered).  A point that a schedule does not pass stays 0.
+constexpr int NSTAMP = 8;
+constexpr const char* PHASE_NAMES = "top,p0_band,last_band,issued,drained,epilogue";
+
+__device__ __forceinline__ uint64_t globaltimer() {
+  uint64_t v;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(v));
+  return v;
+}
 
 
 // Shared memory: [npairs x 9 x 8 KB] weights (resident for the whole kernel) | [NB x band_alloc] activation bands |
 // [2 x 8 KB] bf16 output staging, one 64-row block per consumer warpgroup (BF16OUT only) | barriers.  The MMA issue loop stays free of waits: both pairs' weights are resident rather than streamed through a
 // ring with a wait per tap, and two bands are in flight.
-template <int NB, bool BF16OUT>
+template <int NB, bool BF16OUT, bool PHASES>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_constant__ HaloArgs G) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -126,13 +142,100 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
   const uint32_t w16 = (smem_u32(wsm) & 0x3FFFF) >> 4, band16_0 = (smem_u32(bands) & 0x3FFFF) >> 4;
   const uint32_t band16_step = (uint32_t)G.band_alloc >> 4;
   const int64_t HW = (int64_t)G.H * G.W;
+  // Epilogue without divisions: each thread's output rows are a fixed offset rb into the tile plus steps of ST rows
+  // (bf16 copy-out: rows t/8 + 16 it; fp32 NCHW: rows frag_row + 8 h).  The first row's (image, y, x) is found once
+  // per tile and the next ones by adding the step's precomputed (dy, dx) with a carry.
+  constexpr int ST = BF16OUT ? 16 : 8;
+  const int rb = wg * 64 + (BF16OUT ? (t >> 3) : frag_row(t));
+  const int Hp = G.HpWp / G.Wp, sy = ST / G.Wp, sx = ST - sy * G.Wp;
+  // this thread's 16 output channels' bias, read once
+  const bool has_bias = G.bias != nullptr;
+  float bz[BN / 4];
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+    for (int e = 0; e < 2; ++e) bz[2 * j + e] = has_bias ? G.bias[8 * j + frag_col(t) + e] : 0.f;
   mbar_wait(wfull, 0);
+  unsigned long long* ph = nullptr;
+  if constexpr (PHASES) {
+    ph = G.phases + 4 * gridDim.x + ((size_t)blockIdx.x * G.phase_slots * 2 + wg) * NSTAMP;
+    if (tid == 0) { G.phases[4 * blockIdx.x] = globaltimer(); G.phases[4 * blockIdx.x + 1] = clock64(); }
+  }
+  auto stamp = [&](int slot, int k) {
+    if constexpr (PHASES) { if (t == 0) ph[(size_t)slot * 2 * NSTAMP + k] = clock64(); }
+  };
+
+  // ---------------- epilogue: d[4j + 2h + e] = (row frag_row + 8h, channel 8j + frag_col + e) ----------------
+  auto epilogue = [&](float (&a)[BN / 2], int tile) {
+    int row = tile * BM + rb;   // padded-linear pixel index of this thread's first row
+    int img = (int)((unsigned)row / (unsigned)G.HpWp);
+    int yy = row - img * G.HpWp;
+    int xx = yy;
+    yy = (int)((unsigned)yy / (unsigned)G.Wp);
+    xx -= yy * G.Wp;
+    auto next_row = [&]() {
+      row += ST; xx += sx; yy += sy;
+      if (xx >= G.Wp) { xx -= G.Wp; ++yy; }
+      if (yy >= Hp) { yy -= Hp; ++img; }
+    };
+    if constexpr (BF16OUT) {
+      // bf16 padded-NHWC output: this warpgroup's 64 rows are one contiguous 8 KB block of the output.  Stored from the
+      // fragments, each warp store would cover eight half sectors; staged in shared memory (16-byte chunk j of row r at
+      // r*128 + 16 (j ^ (r & 7)), free of bank conflicts) it goes out as whole 16-byte chunks, border rows as zeros.
+      uint8_t* st = stg + wg * STG_BYTES;
+      named_barrier_sync(1 + wg, 128);    // per warpgroup; the previous tile's copy-out has read the staging block
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int r = frag_row(t) + 8 * h;
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          float f0 = a[4 * j + 2 * h], f1 = a[4 * j + 2 * h + 1];
+          if (has_bias) { f0 += bz[2 * j]; f1 += bz[2 * j + 1]; }
+          *reinterpret_cast<__nv_bfloat162*>(st + r * 128 + 16 * (j ^ (r & 7)) + 2 * frag_col(t)) = __floats2bfloat162_rn(f0, f1);
+        }
+      }
+      named_barrier_sync(1 + wg, 128);
+#pragma unroll
+      for (int it = 0; it < 4; ++it) {
+        const int r = (t >> 3) + 16 * it, c = t & 7;
+        if (row >= G.total_rows) break;
+        uint4 v = make_uint4(0u, 0u, 0u, 0u);
+        if ((unsigned)(yy - 1) < (unsigned)G.H && (unsigned)(xx - 1) < (unsigned)G.W)
+          v = *reinterpret_cast<const uint4*>(st + r * 128 + 16 * (c ^ (r & 7)));
+        *reinterpret_cast<uint4*>(G.out_bf16 + (int64_t)row * 64 + 8 * c) = v;
+        next_row();
+      }
+    } else {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (row < G.total_rows && (unsigned)(yy - 1) < (unsigned)G.H && (unsigned)(xx - 1) < (unsigned)G.W) {
+          float* q = G.out + (int64_t)img * BN * HW + (int64_t)(yy - 1) * G.W + (xx - 1);
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int n = 8 * j + frag_col(t) + e;
+              float v = a[4 * j + 2 * h + e];
+              if (has_bias) v += bz[2 * j + e];
+              float* d = q + (int64_t)n * HW;
+              *d = G.beta ? *d + v : v;
+            }
+          }
+        }
+        next_row();
+      }
+    }
+  };
+
   float acc[BN / 2];
-  int git = 0;
-  for (int tile = blockIdx.x; tile < G.ntiles; tile += gridDim.x) {
+  int git = 0, lt = 0;
+  for (int tile = blockIdx.x; tile < G.ntiles; tile += gridDim.x, ++lt) {
+    stamp(lt, 0);
     for (int p = 0; p < G.npairs; ++p, ++git) {
       const int b = git % NB;
       mbar_wait(bfull0 + 8 * b, (git / NB) & 1);
+      if (p == 0) stamp(lt, 1);
+      if (p == G.npairs - 1) stamp(lt, 2);
       const uint32_t band16 = band16_0 + (uint32_t)b * band16_step;
       const uint32_t wp16 = w16 + (uint32_t)p * (9 * W_TILE >> 4);
       fence_acc(acc);
@@ -145,67 +248,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
           wgmma_n64<0, 0>(acc, dhi | (uint64_t)(alo + 2 * k), dhi | (uint64_t)(blo + 2 * k), (p > 0 || q > 0 || k > 0) ? 1u : 0u);
       }
       wgmma_commit();
+      if (p == G.npairs - 1) stamp(lt, 3);
       fence_acc(acc);
       wgmma_wait<1>();
       if (p > 0 && t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
     }
     wgmma_wait<0>();
     fence_acc(acc);
+    stamp(lt, 4);
     if (t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
-    // ---------------- epilogue: d[4j + 2h + e] = (row frag_row + 8h, channel 8j + frag_col + e) ----------------
-    if constexpr (BF16OUT) {
-      // bf16 padded-NHWC output: this warpgroup's 64 rows are one contiguous 8 KB block of the output.  Stored from the
-      // fragments, each warp store would cover eight half sectors; staged in shared memory (16-byte chunk j of row r at
-      // r*128 + 16 (j ^ (r & 7)), free of bank conflicts) it goes out as whole 16-byte chunks, border rows as zeros.
-      uint8_t* st = stg + wg * STG_BYTES;
-      named_barrier_sync(1 + wg, 128);    // per warpgroup; the previous tile's copy-out has read the staging block
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = frag_row(t) + 8 * h;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int n = 8 * j + frag_col(t);
-          float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
-          if (G.bias) { f0 += G.bias[n]; f1 += G.bias[n + 1]; }
-          *reinterpret_cast<__nv_bfloat162*>(st + r * 128 + 16 * (j ^ (r & 7)) + 2 * frag_col(t)) = __floats2bfloat162_rn(f0, f1);
-        }
-      }
-      named_barrier_sync(1 + wg, 128);
-#pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const int k = t + 128 * it, r = k >> 3, c = k & 7;
-        const int64_t row = (int64_t)tile * BM + wg * 64 + r;   // padded-linear pixel index
-        if (row >= G.total_rows) break;
-        const int img = (int)(row / G.HpWp);
-        const int rem = (int)(row - (int64_t)img * G.HpWp);
-        const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
-        uint4 v = make_uint4(0u, 0u, 0u, 0u);
-        if (yy >= 1 && yy <= G.H && xx >= 1 && xx <= G.W) v = *reinterpret_cast<const uint4*>(st + r * 128 + 16 * (c ^ (r & 7)));
-        *reinterpret_cast<uint4*>(G.out_bf16 + row * 64 + 8 * c) = v;
-      }
-    } else {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t row = (int64_t)tile * BM + wg * 64 + frag_row(t) + 8 * h;   // padded-linear pixel index
-        if (row >= G.total_rows) continue;
-        const int img = (int)(row / G.HpWp);
-        const int rem = (int)(row - (int64_t)img * G.HpWp);
-        const int yy = rem / G.Wp, xx = rem - yy * G.Wp;
-        if (yy < 1 || yy > G.H || xx < 1 || xx > G.W) continue;
-        float* q = G.out + (int64_t)img * BN * HW + (int64_t)(yy - 1) * G.W + (xx - 1);
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int n = 8 * j + frag_col(t) + e;
-            float v = acc[4 * j + 2 * h + e];
-            if (G.bias) v += G.bias[n];
-            float* d = q + (int64_t)n * HW;
-            *d = G.beta ? *d + v : v;
-          }
-        }
-      }
-    }
+    epilogue(acc, tile);
+    stamp(lt, 5);
+  }
+  if constexpr (PHASES) {
+    named_barrier_sync(3, 256);   // ids 1 and 2 are the warpgroups' epilogue barriers
+    if (tid == 0) { G.phases[4 * blockIdx.x + 2] = globaltimer(); G.phases[4 * blockIdx.x + 3] = clock64(); }
   }
 }
 
@@ -378,8 +435,12 @@ bool bb_conv_halo_ok(int C, int O, int H, int W) {
   return !off && C == 64 && O == 64 && W >= 4 && 128 + 2 * (W + 2) + 2 <= BAND_ROWS && H >= 1;
 }
 
-int bb_conv_halo_run(int N, int H, int W, int npairs, const void* const* act_padded, const void* const* wmat, int flip,
-                     float* out, int beta, const float* bias, cudaStream_t s, void* out_bf16_padded) {
+namespace {
+// Launches conv_halo_kernel; with `phases` set, the phase-timing variant (bf16 output only) writes its stamps there.
+// layout (optional) receives {grid, tile slots per CTA, NSTAMP}.
+int conv_halo_launch(int N, int H, int W, int npairs, const void* const* act_padded, const void* const* wmat, int flip,
+                     float* out, int beta, const float* bias, cudaStream_t s, void* out_bf16_padded,
+                     unsigned long long* phases, int* layout) {
   if (npairs < 1 || npairs > 2 || !bb_conv_halo_ok(64, 64, H, W)) return BB_ERR_UNSUPPORTED;
   alignas(64) HaloArgs G;
   memset(&G, 0, sizeof(G));
@@ -408,21 +469,34 @@ int bb_conv_halo_run(int N, int H, int W, int npairs, const void* const* act_pad
   G.nband = nb;
   const size_t smem = fixed + (size_t)nb * G.band_alloc;
   const int grid = G.ntiles < BB_SM_COUNT ? G.ntiles : BB_SM_COUNT;
-  static BbOncePerDevice configured[4];
+  G.phase_slots = (G.ntiles + grid - 1) / grid + 1;
+  if (layout) { layout[0] = grid; layout[1] = G.phase_slots; layout[2] = NSTAMP; }
+  if (layout && !phases) return BB_OK;
+  G.phases = phases;
+  if (phases && !bf) return BB_ERR_ARG;
+  static BbOncePerDevice configured[6];
   auto launch = [&](auto kern, int slot) -> int {
     if (configured[slot].need())
       BB_CUDA_TRY(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     kern<<<grid, NTHREADS, smem, s>>>(G);
     return BB_OK;
   };
-  if (nb == 4)
-    rc = bf ? launch(conv_halo_kernel<4, true>, 0) : launch(conv_halo_kernel<4, false>, 1);
+  if (phases)
+    rc = nb == 4 ? launch(conv_halo_kernel<4, true, true>, 4) : launch(conv_halo_kernel<2, true, true>, 5);
+  else if (nb == 4)
+    rc = bf ? launch(conv_halo_kernel<4, true, false>, 0) : launch(conv_halo_kernel<4, false, false>, 1);
   else
-    rc = bf ? launch(conv_halo_kernel<2, true>, 2) : launch(conv_halo_kernel<2, false>, 3);
+    rc = bf ? launch(conv_halo_kernel<2, true, false>, 2) : launch(conv_halo_kernel<2, false, false>, 3);
   if (rc) return rc;
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
   return BB_OK;
+}
+}  // namespace
+
+int bb_conv_halo_run(int N, int H, int W, int npairs, const void* const* act_padded, const void* const* wmat, int flip,
+                     float* out, int beta, const float* bias, cudaStream_t s, void* out_bf16_padded) {
+  return conv_halo_launch(N, H, W, npairs, act_padded, wmat, flip, out, beta, bias, s, out_bf16_padded, nullptr, nullptr);
 }
 
 // C-ABI hook for the unit test (tests/test_conv_halo_gpu.py)
@@ -439,6 +513,26 @@ extern "C" int bb_conv_halo_bf16_nhwc(int N, int H, int W, int npairs, const voi
   const void* acts[2] = {act0, act1};
   const void* ws[2] = {w0, w1};
   return bb_conv_halo_run(N, H, W, npairs, acts, ws, flip, nullptr, 0, bias, (cudaStream_t)stream, out_padded);
+}
+
+// Phase timing of the bf16 padded-NHWC product (tools/halo_phases.py).  With stamps == NULL only layout is filled:
+// {grid, tile slots per CTA, stamps per slot}; stamps then needs 4 * grid + grid * slots * 2 * NSTAMP entries, zeroed.
+extern "C" int bb_conv_halo_phases(int N, int H, int W, int npairs, const void* act0, const void* act1, const void* w0,
+                                   const void* w1, int flip, void* out_padded, const float* bias,
+                                   unsigned long long* stamps, int* layout, void* stream) {
+  if (layout == nullptr) return BB_ERR_ARG;
+  const void* acts[2] = {act0, act1};
+  const void* ws[2] = {w0, w1};
+  return conv_halo_launch(N, H, W, npairs, acts, ws, flip, nullptr, 0, bias, (cudaStream_t)stream, out_padded, stamps,
+                          layout);
+}
+
+// names of the stamp points of bb_conv_halo_phases, comma-separated, in the order of k
+extern "C" int bb_conv_halo_phase_names(char* buf, int cap) {
+  const int n = (int)strlen(PHASE_NAMES);
+  if (buf == nullptr || cap <= n) return BB_ERR_ARG;
+  memcpy(buf, PHASE_NAMES, n + 1);
+  return BB_OK;
 }
 
 int bb_wgrad_halo_run(int N, int H, int W, int C, int O, int npairs, const void* const* x_padded, const void* const* gy_padded,

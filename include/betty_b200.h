@@ -137,6 +137,12 @@ int bb_conv_halo_bf16(int N, int H, int W, int npairs, const void* act0, const v
 int bb_conv_halo_bf16_nhwc(int N, int H, int W, int npairs, const void* act0, const void* act1, const void* w0,
                            const void* w1, int flip, void* out_padded /* bf16 [N][H+2][W+2][64] */, const float* bias,
                            void* stream);
+/* phase timing of the bf16 padded-NHWC product (tools/halo_phases.py): a separate instantiation writes clock64 stamps
+ * at the points bb_conv_halo_phase_names lists; with stamps == NULL only layout = {grid, tile slots per CTA, stamps per
+ * slot} is filled, and stamps then needs 4*grid + grid*slots*2*stamps_per_slot zeroed entries */
+int bb_conv_halo_phases(int N, int H, int W, int npairs, const void* act0, const void* act1, const void* w0, const void* w1,
+                        int flip, void* out_padded, const float* bias, unsigned long long* stamps, int* layout, void* stream);
+int bb_conv_halo_phase_names(char* buf, int cap);
 /* weight-gradient companion (wgrad_halo_kernel): out[o][c][tap] (fp32 [64][64][9], accumulated) +=
  * sum_pixels gy[pixel][o] * x[pixel + d(tap)][c], x / gy bf16 padded NHWC */
 int bb_wgrad_halo_bf16(int N, int H, int W, int npairs, const void* x0, const void* x1, const void* g0, const void* g1,
