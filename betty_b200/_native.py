@@ -52,6 +52,9 @@ _SIGS = {
     "bb_gemm_bf16_tma": ([C.c_int64, C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_int64, C.c_int64, C.c_void_p, C.c_int,
                           C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
                           C.c_void_p], None),
+    "bb_gemm_bf16_tma_ex": ([C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                             C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_int64,
+                             C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p], None),
     "bb_plan_set_scratch": ([C.c_void_p, C.c_void_p, C.c_int64], 0),
     "bb_plan_set_persistent": ([C.c_void_p, C.c_void_p, C.c_int64], 0),
     "bb_node_bytes": ([], 0),

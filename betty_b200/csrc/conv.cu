@@ -347,7 +347,7 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     }
     G.npairs = np;
     G.out = reinterpret_cast<float*>(base ? nd.a[1] : nd.at[1]); G.omode = 0; G.ors = 1; G.ocs = CKK;
-    G.beta = 1; G.bias = nullptr; G.allow_split = 1; G.out_dense = 1;
+    G.beta = 1; G.bias = nullptr; G.allow_split = 1;
     rc = bb_gemm_tc_run(G, s);
     if (rc) return rc;
   } else if ((need & 2) && unit && bb_conv_small_wgrad_ok(g.O, g.C, g.H, g.W, g.HO, g.WO, g.KH, g.KW)) {

@@ -109,7 +109,6 @@ int run_gemm(int64_t M, int64_t N, int64_t K, int64_t batch, int npairs, const M
     }
     G.out = out; G.omode = 0; G.ors = ors; G.ocs = ocs; G.beta = beta; G.bias = bias; G.bias_stride = bias_stride;
     G.allow_split = 1;
-    G.out_dense = dense_block(M, N, 1, ors, ocs, 0);
     return bb_gemm_tc_run(G, s);
   }
   StridedLoad la{}, lb{};

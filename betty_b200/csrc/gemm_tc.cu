@@ -1,7 +1,7 @@
 // K5 tensor-core path: dual-product GEMM on the Hopper tensor cores (wgmma.mma_async with bf16 operands from
 // shared memory, fp32 accumulation in registers) for the bf16-autocast configurations.
 //
-//   D[m][n] (beta/atomic)= sum over up to two operand pairs p of  sum_k A_p[m][k] * B_p[k][n]   (+ bias[n])
+//   D[m][n] (beta)= sum over up to two operand pairs p of  sum_k A_p[m][k] * B_p[k][n]   (+ bias[n])
 //
 // Operand staging is done by the threads themselves rather than by TMA because the second-order operands are
 // heterogeneous: base activations / weights are bf16 (autocast), tangents and adjoints are fp32 slices of arenas,
@@ -11,7 +11,7 @@
 // the stage with a generic->async proxy fence and a CTA barrier.  Each of the two warpgroups then issues
 // 4 x wgmma m64nBNk16 per 64-wide k-block for its 64 rows of the 128-row tile; the MMAs of k-block i run while
 // k-block i+1 is staged (3-stage ring, wait_group 1).  The epilogue stores the register accumulators with beta /
-// atomic split-K / bias handling.
+// bias handling, or, under split-K, into per-split partials that bb_splitk_finish adds in split order.
 //
 // 256 threads = 2 warpgroups, 24-32 KB per stage.
 #include <cuda_bf16.h>
@@ -22,6 +22,7 @@
 #include "gemm_tc.h"
 #include "plan.h"
 #include "tc_ptx.cuh"
+#include "tma.h"
 
 namespace {
 
@@ -464,10 +465,13 @@ __global__ void __launch_bounds__(NTHREADS, MINB) gemm_tc_kernel(const __grid_co
         const int64_t col = n0 + 8 * j + frag_col(t) + e;
         if (col < G.N) {
           float v = acc[4 * j + 2 * h + e];
-          if (G.bias != nullptr && split == 0) v += G.bias[col * G.bias_stride];
+          if (G.part != nullptr) {   // split-K: bias and beta are applied when the partials are added
+            G.part[((int64_t)split * G.M + row) * G.N + col] = v;
+            continue;
+          }
+          if (G.bias != nullptr) v += G.bias[col * G.bias_stride];
           float* dst = G.out + row_base + col * col_stride;
-          if (G.ksplit > 1) atomicAdd(dst, v);
-          else *dst = G.beta ? *dst + v : v;
+          *dst = G.beta ? *dst + v : v;
         }
       }
     }
@@ -506,15 +510,19 @@ int bb_gemm_tc_run(const TcGemmArgs& G0, cudaStream_t s) {
     if (ksplit > 64) ksplit = 64;
     if (ksplit < 1) ksplit = 1;
   }
-  if (ksplit > 1 && !G.beta) {
-    if (!G.out_dense) {
-      ksplit = 1;
-    } else {
-      BB_CUDA_TRY(cudaMemsetAsync(G.out, 0, sizeof(float) * G.M * G.N, s));
-      bb_launch_tally += 1;
-    }
+  // split-K partials go to the plan's reduction workspace (outside a plan: a stream-ordered buffer) and are added in
+  // split order by bb_splitk_finish
+  const size_t split_bytes = sizeof(float) * (size_t)G.M * (size_t)G.N;
+  if (ksplit > 1 && bb_reduce_ws.base != nullptr) ksplit = bb_reduce_ws_splits(ksplit, split_bytes);
+  if (ksplit > 1) {   // no empty splits
+    const int64_t kb_per = (kblocks + ksplit - 1) / ksplit;
+    ksplit = (int)((kblocks + kb_per - 1) / kb_per);
   }
   G.ksplit = ksplit;
+  G.part = nullptr;
+  bool owned = false;
+  if (ksplit > 1 && (G.part = bb_partials_acquire(split_bytes * ksplit, s, &owned)) == nullptr)
+    return (int)cudaErrorMemoryAllocation;
   // row-contiguous strided operands (transposed views) are staged MN-major: contiguous 16-byte reads, no transpose
   static const bool no_mn = getenv("BB200_TC_NO_MN") != nullptr;
   for (int p = 0; p < G.npairs; ++p) {
@@ -524,14 +532,22 @@ int bb_gemm_tc_run(const TcGemmArgs& G0, cudaStream_t s) {
   const bool need_lut = G.a[0].mode == TC_PIXROW || G.a[0].mode == TC_WDGRAD || G.b[0].mode == TC_PIXROW ||
                         G.b[0].mode == TC_WDGRAD;
   G.lut_k = need_lut ? (int)G.K : 0;
-  if (G.lut_k > kMaxLutK) return BB_ERR_UNSUPPORTED;
+  if (G.lut_k > kMaxLutK) {
+    bb_partials_release(G.part, owned, s);
+    return BB_ERR_UNSUPPORTED;
+  }
   // Two register budgets are compiled: 1 CTA/SM and, for 64-wide tiles, 2 CTAs/SM (capped at 128 registers).  The convolution gathers
   // are issue-latency bound and gain from a second resident CTA; plain strided GEMMs keep the larger budget.
   static const int forced = getenv("BB200_TC_OCC") ? atoi(getenv("BB200_TC_OCC")) : 0;
   const int occ = forced ? forced : (need_lut || G.a[0].mode == TC_PIXK ? 2 : 1);
   // (128 accumulator registers of a 128-wide tile do not fit the 2-CTA budget: those tiles always run one per SM)
-  if (occ >= 2 && bn == 64) return launch_tc<64, 2>(G, ksplit, s);
-  return bn == 64 ? launch_tc<64, 1>(G, ksplit, s) : launch_tc<128, 1>(G, ksplit, s);
+  int rc = (occ >= 2 && bn == 64) ? launch_tc<64, 2>(G, ksplit, s)
+           : bn == 64             ? launch_tc<64, 1>(G, ksplit, s)
+                                  : launch_tc<128, 1>(G, ksplit, s);
+  if (rc == BB_OK && G.part != nullptr)
+    rc = bb_splitk_finish(G.part, ksplit, G.M, G.N, false, G.out, G.ors, G.ocs, G.beta, G.bias, G.bias_stride, s);
+  bb_partials_release(G.part, owned, s);
+  return rc;
 }
 
 extern "C" int bb_gemm_bf16_tc(int64_t M, int64_t N, int64_t K, const void* A, int dtA, int64_t ars, int64_t acs,
@@ -543,6 +559,5 @@ extern "C" int bb_gemm_bf16_tc(int64_t M, int64_t N, int64_t K, const void* A, i
   G.b[0] = tc_strided(B, dtB, bcs, brs);   // B tile rows = n: elem(n,k) = B[k*brs + n*bcs]
   G.out = C; G.omode = 0; G.ors = crs; G.ocs = ccs; G.beta = beta; G.bias = nullptr; G.bias_stride = 0;
   G.allow_split = 1;
-  G.out_dense = (ccs == 1 && crs == N) || (crs == 1 && ccs == M);
   return bb_gemm_tc_run(G, (cudaStream_t)stream);
 }

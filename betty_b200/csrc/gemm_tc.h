@@ -32,8 +32,9 @@ struct TcGemmArgs {
   int beta;
   const float* bias; // indexed by n
   int64_t bias_stride;
-  int allow_split, out_dense;
+  int allow_split;
   int lut_k;         // set by bb_gemm_tc_run: entries of the k -> gather-offset tables (0 if unused)
+  float* part;       // set by bb_gemm_tc_run when ksplit > 1: split sp writes its partial to part[(sp*M + m)*N + n]
 };
 
 inline TcSrc tc_strided(const void* p, int dt, int64_t rs, int64_t cs) {

@@ -1,7 +1,7 @@
 // K5/K6 tensor-core path, TMA-fed: dual-product GEMM and stride-1 convolution (forward / input-gradient form) on
 // wgmma.mma_async with operands brought into shared memory by the TMA unit.
 //
-//   D[m][n] (beta/atomic)= sum over up to two operand pairs p of  sum_k A_p[m][k] * B_p[n][k]   (+ bias[n])
+//   D[m][n] (beta)= sum over up to two operand pairs p of  sum_k A_p[m][k] * B_p[n][k]   (+ bias[n])
 //
 // The software-staged kernel in gemm_tc.cu spends most of its time staging operands (address arithmetic, 4-byte
 // gathers, bf16 conversion, swizzled stores).  Here every operand is first made TMA-addressable -- bf16, unit stride
@@ -60,7 +60,14 @@ struct Cfg {
 struct OutRows {
   int omode, img, h0;
   int64_t m0, bz;
+  int split;
   __device__ __forceinline__ bool map(const TmaGemmArgs& G, int r, int64_t* base, int64_t* col_stride) const {
+    if (G.part != nullptr) {   // split-K partial (omode 0, no batch)
+      const int64_t row = m0 + r;
+      *base = (int64_t)split * G.M * G.N + row * G.prs;
+      *col_stride = G.pcs;
+      return row < G.M;
+    }
     if (omode == 1) {
       const int64_t q = (int64_t)h0 * G.Wb + r;   // Wb == output width
       *base = (int64_t)img * G.OCH * G.OHW + q;
@@ -85,8 +92,12 @@ struct OutRows {
 template <int BN_>
 __device__ __forceinline__ void epi_store(const TmaGemmArgs& G, const float (&acc)[BN_ / 2], const OutRows& R, int wg, int t,
                                           int n0, bool add_bias) {
-  const bool vec = G.omode == 0 && G.ocs == 1 && (G.ors & 1) == 0 && (G.obs & 1) == 0 &&
-                   ((reinterpret_cast<uintptr_t>(G.out) & 7) == 0) && G.ksplit == 1;
+  const bool to_part = G.part != nullptr;
+  const bool vec = to_part ? G.pcs == 1 && (G.N & 1) == 0
+                           : G.omode == 0 && G.ocs == 1 && (G.ors & 1) == 0 && (G.obs & 1) == 0 &&
+                                 ((reinterpret_cast<uintptr_t>(G.out) & 7) == 0);
+  float* const dst = to_part ? G.part : G.out;
+  const bool accumulate = G.beta && !to_part;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     int64_t base, cs;
@@ -101,19 +112,16 @@ __device__ __forceinline__ void epi_store(const TmaGemmArgs& G, const float (&ac
         v0 += G.bias[(int64_t)col * G.bias_stride];
         if (two) v1 += G.bias[(int64_t)(col + 1) * G.bias_stride];
       }
-      float* q = G.out + base + (int64_t)col * cs;
+      float* q = dst + base + (int64_t)col * cs;
       if (vec && two) {
         float2* q2 = reinterpret_cast<float2*>(q);
         float2 o = make_float2(v0, v1);
-        if (G.beta) {
+        if (accumulate) {
           const float2 old = *q2;
           o.x += old.x; o.y += old.y;
         }
         *q2 = o;
-      } else if (G.ksplit > 1) {
-        atomicAdd(q, v0);
-        if (two) atomicAdd(q + cs, v1);
-      } else if (G.beta) {
+      } else if (accumulate) {
         *q += v0;
         if (two) q[cs] += v1;
       } else {
@@ -239,8 +247,8 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_kernel(const __grid_cons
     }
     wgmma_wait<0>();
     fence_acc(acc);
-    const OutRows R{G.omode, img, h0, (int64_t)m0, (int64_t)bz};
-    epi_store<BN_>(G, acc, R, wg, t, n0, G.bias != nullptr && split == 0);
+    const OutRows R{G.omode, img, h0, (int64_t)m0, (int64_t)bz, split};
+    epi_store<BN_>(G, acc, R, wg, t, n0, G.bias != nullptr && G.part == nullptr);
   }
 }
 
@@ -317,7 +325,7 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_persist_kernel(const __g
       wgmma_wait<0>();
       fence_acc(acc);
       if (t == 0) mbar_arrive(empty0 + 8 * ((git - 1) % STAGES));
-      OutRows R{G.omode, 0, 0, (int64_t)mt * BM, 0};
+      OutRows R{G.omode, 0, 0, (int64_t)mt * BM, 0, 0};
       if (conv) {
         R.img = mt / G.tiles_per_img;
         R.h0 = (mt - R.img * G.tiles_per_img) * G.Hb;
@@ -327,8 +335,26 @@ __global__ void __launch_bounds__(NTHREADS, 2) gemm_tma_persist_kernel(const __g
   }
 }
 
+// Second half of a split-K product (bb_splitk_finish, tma.h).  Threads walk the partials' dense layout, so the reads
+// (and the writes when the output has the same layout) coalesce.
+__global__ void __launch_bounds__(256) splitk_finish_kernel(const float* __restrict__ part, int ksplit, int64_t M,
+                                                            int64_t N, bool col_major, float* out, int64_t ors,
+                                                            int64_t ocs, int beta, const float* __restrict__ bias,
+                                                            int64_t bias_stride) {
+  const int64_t mn = M * N;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < mn; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t hi = col_major ? i / M : i / N, lo = col_major ? i - hi * M : i - hi * N;
+    const int64_t m = col_major ? lo : hi, n = col_major ? hi : lo;
+    float v = 0.f;
+    for (int sp = 0; sp < ksplit; ++sp) v += part[sp * mn + i];
+    if (bias != nullptr) v += bias[n * bias_stride];
+    float* q = out + m * ors + n * ocs;
+    *q = beta ? *q + v : v;
+  }
+}
+
 template <int BN_>
-int launch_tma(TmaGemmArgs& G, int64_t mtiles, cudaStream_t s, int batch) {
+int launch_tma(TmaGemmArgs& G, int64_t mtiles, cudaStream_t s, int batch, bool persistent, bool* launched_persistent) {
   using C = Cfg<BN_>;
   static BbOncePerDevice configured;
   if (configured.need()) {
@@ -344,7 +370,9 @@ int launch_tma(TmaGemmArgs& G, int64_t mtiles, cudaStream_t s, int batch) {
   G.stages = ctas <= BB_SM_COUNT ? C::kStagesDeep : C::kStagesShared;
   if (forced >= 2 && forced <= C::kStagesDeep) G.stages = forced;
   static const bool no_persist = getenv("BB200_TMA_NO_PERSIST") != nullptr;
-  if (!no_persist && G.ksplit == 1 && batch == 1 && ctas > 4 * BB_SM_COUNT) {
+  const bool persist = persistent && !no_persist && G.ksplit == 1 && batch == 1 && ctas > 4 * BB_SM_COUNT;
+  if (launched_persistent) *launched_persistent = persist;
+  if (persist) {
     static BbOncePerDevice configured_p;
     if (configured_p.need()) {
       BB_CUDA_TRY(cudaFuncSetAttribute(gemm_tma_persist_kernel<BN_>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -706,8 +734,21 @@ int bb_pack_im2col(const void* src, int dt, const Im2colGeom& g, void* dst, int 
   return BB_OK;
 }
 
-int bb_gemm_tma_launch(TmaGemmArgs& G, int bn, int64_t mtiles, cudaStream_t s, int batch) {
-  return bn == 64 ? launch_tma<64>(G, mtiles, s, batch) : launch_tma<128>(G, mtiles, s, batch);
+int bb_splitk_finish(const float* part, int ksplit, int64_t M, int64_t N, bool col_major, float* out, int64_t ors,
+                     int64_t ocs, int beta, const float* bias, int64_t bias_stride, cudaStream_t s) {
+  int64_t blocks = (M * N + 255) / 256;
+  if (blocks > 4 * BB_SM_COUNT) blocks = 4 * BB_SM_COUNT;
+  splitk_finish_kernel<<<(unsigned)blocks, 256, 0, s>>>(part, ksplit, M, N, col_major, out, ors, ocs, beta, bias,
+                                                        bias_stride);
+  bb_launch_tally += 1;
+  BB_LAUNCH_CHECK();
+  return BB_OK;
+}
+
+int bb_gemm_tma_launch(TmaGemmArgs& G, int bn, int64_t mtiles, cudaStream_t s, int batch, bool persistent,
+                       bool* launched_persistent) {
+  return bn == 64 ? launch_tma<64>(G, mtiles, s, batch, persistent, launched_persistent)
+                  : launch_tma<128>(G, mtiles, s, batch, persistent, launched_persistent);
 }
 
 int bb_gemm_tma_prepack(const TmaPackReq* reqs, int n, int64_t batch, cudaStream_t s) {
@@ -730,7 +771,7 @@ int bb_gemm_tma_prepack(const TmaPackReq* reqs, int n, int64_t batch, cudaStream
 
 int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* A, const TmaView* B, float* out,
                     int64_t ors, int64_t ocs, int beta, const float* bias, int64_t bias_stride, bool out_dense,
-                    cudaStream_t s, int plane_ohw, int min_n, int64_t batch, int64_t obs) {
+                    cudaStream_t s, int plane_ohw, int min_n, int64_t batch, int64_t obs, int flags, int* route) {
   if (npairs < 1 || npairs > 2 || batch < 1) return BB_DECLINED;
   if (batch == 1) {
     if (M < 64 || N < min_n || K < 8) return BB_DECLINED;
@@ -752,10 +793,20 @@ int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* 
   memset(&G, 0, sizeof(G));
   // Tile width and split-K by a cost model.  The kernel is bound by what one SM can pull through the TMA unit (a
   // 128 x bn x 64 k-block costs 16 + bn/8 KB), so the time of a configuration is (waves of CTAs) x (k-blocks per CTA)
-  // x (bytes per k-block) / per-SM rate; split-K adds a memset launch and the reduction traffic of its partial tiles.
+  // x (bytes per k-block) / per-SM rate; split-K adds a launch (when not accumulating) and the traffic of its partials.
+  // The partials of these shapes stay in L2: charging their read-back and the extra launch at HBM rates made the model
+  // stop splitting RoBERTa's 800 x 768 two-pair products, and the benchmark's bert_data_reweighting line fell from
+  // 73.4-74.0 to 67.4-68.1 HVP-it/s (H100 SXM 80 GB, 700 W), so the charge is the one the atomic finish had.  Inside
+  // a plan the partials must fit the plan's reduction workspace.
   const int64_t mtiles = (M + BM - 1) / BM;
   const int64_t kblocks = (K + BK - 1) / BK;
   const bool can_split = batch == 1 && plane_ohw == 0 && (beta || out_dense) && kblocks >= 8;
+  const size_t split_bytes = sizeof(float) * (size_t)M * (size_t)N;
+  const int max_split = bb_reduce_ws.base != nullptr ? bb_reduce_ws_splits(256, split_bytes) : 256;
+  const int force_bn = (flags & TMA_FORCE_BN64) ? 64 : (flags & TMA_FORCE_BN128) ? 128 : 0;
+  const int force_split = (flags >> 8) & 255;
+  if (force_bn == 128 && N <= 64) return BB_DECLINED;
+  if (force_split > 1 && (!can_split || force_split > kblocks)) return BB_DECLINED;
   int bn = 64, ksplit = 1;
   {
     double best = 1e30;
@@ -763,14 +814,15 @@ int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* 
     for (int bi = 0; bi < 2; ++bi) {
       const int cand = bn_opts[bi];
       if (cand == 128 && N <= 64) continue;
+      if (force_bn && cand != force_bn) continue;
       const int64_t tiles = mtiles * ((N + cand - 1) / cand) * batch;
       for (int sp = 1; sp <= 256; sp = sp < 4 ? sp + 1 : sp * 2) {
-        if (sp > 1 && (!can_split || kblocks / sp < 4)) break;
+        if (sp > 1 && (!can_split || kblocks / sp < 4 || sp > max_split)) break;
         const int64_t ctas = tiles * sp;
         const int64_t waves = (ctas + BB_SM_COUNT - 1) / BB_SM_COUNT;
         const int64_t iters = (kblocks + sp - 1) / sp * npairs;
         double us = (double)waves * (double)iters * (16.0 + cand / 8.0) * 1024.0 / 84e3 + 2.0;   // 84 GB/s per SM
-        if (sp > 1) us += (beta ? 0.0 : 2.5) + (double)M * (double)N * 4.0 * sp / 2.0e6;          // ~2 TB/s of reductions
+        if (sp > 1) us += (beta ? 0.0 : 2.5) + (double)split_bytes * sp / 2.0e6;                 // see above
         if (us < best) {
           best = us;
           bn = cand;
@@ -778,6 +830,12 @@ int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* 
         }
       }
     }
+  }
+  if (force_split) ksplit = force_split;
+  {
+    // no empty splits: every split owns at least one k-block
+    const int64_t kb_per = (kblocks + ksplit - 1) / ksplit;
+    ksplit = (int)((kblocks + kb_per - 1) / kb_per);
   }
   PackJobs J{};
   Prepared pa[2], pb[2];
@@ -807,12 +865,30 @@ int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* 
   if (plane_ohw > 0) {
     G.omode = 2; G.OCH = (int)N; G.OHW = plane_ohw;
   }
-  if (ksplit > 1 && !beta) {
-    BB_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * M * N, s));
-    bb_launch_tally += 1;
-  }
   G.ksplit = ksplit;
-  return bb_gemm_tma_launch(G, bn, mtiles, s, (int)batch);
+  if (route) {
+    route[0] = bn; route[1] = ksplit; route[2] = 0;
+    for (int p = 0; p < 2; ++p) {
+      route[3 + 2 * p] = p < npairs ? G.a_kind[p] : -1;
+      route[4 + 2 * p] = p < npairs ? G.b_kind[p] : -1;
+    }
+  }
+  if (ksplit == 1) {
+    bool persistent = false;
+    const int rc = bb_gemm_tma_launch(G, bn, mtiles, s, (int)batch, !(flags & TMA_NO_PERSIST), &persistent);
+    if (route) route[2] = persistent ? 1 : 0;
+    return rc;
+  }
+  bool owned = false;
+  G.part = bb_partials_acquire(split_bytes * ksplit, s, &owned);
+  if (G.part == nullptr) return (int)cudaErrorMemoryAllocation;
+  const bool col_major = ors == 1 && ocs != 1;   // partials in the output's own order: the finishing writes coalesce
+  G.prs = col_major ? 1 : N;
+  G.pcs = col_major ? M : 1;
+  int rc = bb_gemm_tma_launch(G, bn, mtiles, s, 1);
+  if (rc == BB_OK) rc = bb_splitk_finish(G.part, ksplit, M, N, col_major, out, ors, ocs, beta, bias, bias_stride, s);
+  bb_partials_release(G.part, owned, s);
+  return rc;
 }
 
 extern "C" int bb_gemm_bf16_tma(int64_t M, int64_t N, int64_t K, const void* A, int dtA, int64_t ars, int64_t acs,
@@ -824,6 +900,30 @@ extern "C" int bb_gemm_bf16_tma(int64_t M, int64_t N, int64_t K, const void* A, 
   const TmaView a{A, dtA, ars, acs}, b{B, dtB, bcs, brs};   // rows of the B view = n
   const bool dense = (ccs == 1 && crs == N) || (crs == 1 && ccs == M);
   const int rc = bb_gemm_tma_run(M, N, K, 1, &a, &b, C, crs, ccs, beta, nullptr, 0, dense, (cudaStream_t)stream);
+  bb_scratch = saved;
+  bb_scratch_reset();
+  return rc;
+}
+
+extern "C" int bb_gemm_bf16_tma_ex(int64_t M, int64_t N, int64_t K, int npairs, int64_t batch, const void* const* A,
+                                   const int64_t* a_desc, const void* const* B, const int64_t* b_desc, float* C,
+                                   int64_t crs, int64_t ccs, int64_t cbs, int beta, const float* bias,
+                                   int64_t bias_stride, int plane_ohw, int min_n, int flags, void* scratch,
+                                   int64_t scratch_bytes, int* route, void* stream) {
+  if (npairs < 1 || npairs > 2) return BB_ERR_ARG;
+  TmaView a[2], b[2];
+  for (int p = 0; p < npairs; ++p) {
+    const int64_t* ad = a_desc + 4 * p;
+    const int64_t* bd = b_desc + 4 * p;
+    a[p] = TmaView{A[p], (int)ad[0], ad[1], ad[2], ad[3]};
+    b[p] = TmaView{B[p], (int)bd[0], bd[2], bd[1], bd[3]};   // rows of the B view = n
+  }
+  const BbScratch saved = bb_scratch;
+  bb_scratch = BbScratch{reinterpret_cast<uint8_t*>(scratch), (size_t)scratch_bytes, 0};
+  bb_scratch_reset();
+  const bool dense = (ccs == 1 && crs == N) || (crs == 1 && ccs == M);
+  const int rc = bb_gemm_tma_run(M, N, K, npairs, a, b, C, crs, ccs, beta, bias, bias_stride, dense,
+                                 (cudaStream_t)stream, plane_ohw, min_n, batch, cbs, flags, route);
   bb_scratch = saved;
   bb_scratch_reset();
   return rc;

@@ -19,9 +19,17 @@ struct TmaView {
 // batch > 1: `batch` independent products (operand / output batch strides TmaView::bs / obs), one grid.z slice each.
 // plane_ohw > 0: the rows are pixels (img, q) of planes with plane_ohw pixels and the output is NCHW,
 // out[(img*N + n)*plane_ohw + q] (ors / ocs unused).  min_n: smallest N accepted (64 for Linear layers).
+// Split-K writes one partial product per split into the plan's reduction workspace (outside a plan: a stream-ordered
+// buffer) and a second kernel adds them in split order, so results do not depend on the order the CTAs ran in.
+// flags (unit tests; 0 = the cost model decides): TMA_FORCE_BN64 / TMA_FORCE_BN128, TMA_NO_PERSIST, and a split count
+// in bits 8..15 (TMA_FORCE_KSPLIT(n)).  route, when set, receives the launched configuration: TMA_ROUTE_WORDS ints
+// {bn, ksplit, persistent, a_kind[0], b_kind[0], a_kind[1], b_kind[1]}.
+enum { TMA_FORCE_BN64 = 1, TMA_FORCE_BN128 = 2, TMA_NO_PERSIST = 4, TMA_ROUTE_WORDS = 7 };
+#define TMA_FORCE_KSPLIT(n) ((n) << 8)
 int bb_gemm_tma_run(int64_t M, int64_t N, int64_t K, int npairs, const TmaView* A, const TmaView* B, float* out,
                     int64_t ors, int64_t ocs, int beta, const float* bias, int64_t bias_stride, bool out_dense,
-                    cudaStream_t s, int plane_ohw = 0, int min_n = 64, int64_t batch = 1, int64_t obs = 0);
+                    cudaStream_t s, int plane_ohw = 0, int min_n = 64, int64_t batch = 1, int64_t obs = 0,
+                    int flags = 0, int* route = nullptr);
 
 // Pack, in as few launches as possible (four operands per launch), every listed view that is not TMA-addressable as
 // it stands; the bb_gemm_tma_run calls of the same node then find the packs in the per-node cache.  rows / k as in
@@ -51,9 +59,14 @@ struct alignas(64) TmaGemmArgs {
   int beta;
   const float* bias;
   int64_t bias_stride;
+  float* part;                 // ksplit > 1: split sp writes its partial to part[sp*M*N + m*prs + n*pcs] (no bias, beta)
+  int64_t prs, pcs;
 };
 
-int bb_gemm_tma_launch(TmaGemmArgs& G, int bn, int64_t mtiles, cudaStream_t s, int batch = 1);
+// persistent: may the persistent kernel take the launch (it does when the grid is more than 4 CTAs per SM);
+// *launched_persistent (optional) says whether it did.
+int bb_gemm_tma_launch(TmaGemmArgs& G, int bn, int64_t mtiles, cudaStream_t s, int batch = 1, bool persistent = true,
+                       bool* launched_persistent = nullptr);
 
 // ---- packs (gemm_tma.cu) ----
 // dst[o][i] = bf16(src[o*os + i*is]), o < outer, i < inner; dst pitch dp (>= inner, multiple of 8), tail zero-filled

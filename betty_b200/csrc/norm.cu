@@ -14,6 +14,7 @@
 #include "../../include/betty_b200.h"
 #include "bb_common.cuh"
 #include "plan.h"
+#include "tma.h"
 
 namespace {
 
@@ -227,8 +228,9 @@ __global__ void __launch_bounds__(256) bn_apply_kernel(const __grid_constant__ B
 }
 
 // ---------------------------------------------------------------------------------------------------
-// LayerNorm: one warp per row, statistics recomputed per pass; parameter gradients go through
-// block-level shared-memory column accumulators and one global atomic per column per block.
+// LayerNorm: one warp per row, statistics recomputed per pass.  Parameter adjoints: each block writes its per-column
+// sums to part[block][D] (gamma) and part[gridDim.x + block][D] (beta), and ln_params_finish_kernel adds them in a
+// fixed order, so the result does not depend on the order the blocks ran in.
 // ---------------------------------------------------------------------------------------------------
 struct LnArgs {
   const void* x;
@@ -243,6 +245,7 @@ struct LnArgs {
   float* dst;
   float* at_gamma;
   float* at_beta;
+  float* part;   // BN_TB: [2][gridDim.x][D] per-block partials of at_gamma, at_beta
   int64_t rows;
   int D;
   float eps;
@@ -256,12 +259,13 @@ constexpr int kLnRowsPerWarp = 1;
 
 template <int MODE>  // BN_BB / BN_TF / BN_TB reuse the enum
 __global__ void __launch_bounds__(kLnWarps * 32) ln_kernel(const __grid_constant__ LnArgs A) {
-  extern __shared__ float colacc[];  // [2][D] for MODE == TB
+  extern __shared__ float colsm[];  // [kLnWarps][2][D] for MODE == TB: one slot per warp, added in warp order
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int D = A.D;
+  float* colacc = colsm + (int64_t)warp * 2 * D;
   if (MODE == BN_TB) {
-    for (int c = threadIdx.x; c < 2 * D; c += blockDim.x) colacc[c] = 0.f;
-    __syncthreads();
+    for (int c = lane; c < 2 * D; c += 32) colacc[c] = 0.f;
+    __syncwarp();
   }
   const float invD = 1.f / (float)D;
   for (int rr = 0; rr < kLnRowsPerWarp; ++rr) {
@@ -319,8 +323,8 @@ __global__ void __launch_bounds__(kLnWarps * 32) ln_kernel(const __grid_constant
       const float gh = g * GAM(c), ght = gt * GAM(c) + (A.tgamma ? g * A.tgamma[c] : 0.f);
       b1 += ght;
       b2 += ght * xh + gh * dxh;
-      atomicAdd(&colacc[c], gt * xh + g * dxh);
-      atomicAdd(&colacc[D + c], gt);
+      colacc[c] += gt * xh + g * dxh;
+      colacc[D + c] += gt;
     }
     const float mt1 = bb::warp_sum(b1) * invD, mt2 = bb::warp_sum(b2) * invD;
     for (int c = lane; c < D; c += 32) {
@@ -336,9 +340,12 @@ __global__ void __launch_bounds__(kLnWarps * 32) ln_kernel(const __grid_constant
   }
   if (MODE == BN_TB) {
     __syncthreads();
-    for (int c = threadIdx.x; c < D; c += blockDim.x) {
-      if (A.at_gamma) atomicAdd(A.at_gamma + c, colacc[c]);
-      if (A.at_beta) atomicAdd(A.at_beta + c, colacc[D + c]);
+    for (int c = threadIdx.x; c < 2 * D; c += blockDim.x) {
+      float v = 0.f;
+#pragma unroll
+      for (int w = 0; w < kLnWarps; ++w) v += colsm[w * 2 * D + c];
+      const int half = c >= D;
+      A.part[((int64_t)half * gridDim.x + blockIdx.x) * D + (c - half * D)] = v;
     }
   }
 }
@@ -347,7 +354,7 @@ __global__ void __launch_bounds__(kLnWarps * 32) ln_kernel(const __grid_constant
 // consecutive columns, keeps x / t_x / a_y / at_y of the row in registers (each operand is read once, 128-bit), and
 // the statistics need three block reductions instead of the warp kernel's eight dependent passes over L1:
 //   P1 {sum x, sum t_x}   P2 {sum dx^2, sum dx*dt}   P3 {sum gh, sum gh*xh, sum ght, sum ght*xh + gh*dxh}
-// The per-column parameter adjoints accumulate in registers over the block's rows -> one atomic per column per block.
+// The per-column parameter adjoints accumulate in registers over the block's rows -> one partial per column per block.
 __device__ __forceinline__ void block_sum4(float& a, float& b, float& c, float& d, float (*red)[8]) {
   a = bb::warp_sum(a); b = bb::warp_sum(b); c = bb::warp_sum(c); d = bb::warp_sum(d);
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -469,11 +476,33 @@ __global__ void __launch_bounds__(256) ln_row_kernel(const __grid_constant__ LnA
     }
   }
   if (MODE == BN_TB && on) {
+    *reinterpret_cast<float4*>(A.part + (int64_t)blockIdx.x * D + c0) = make_float4(cg[0], cg[1], cg[2], cg[3]);
+    *reinterpret_cast<float4*>(A.part + ((int64_t)gridDim.x + blockIdx.x) * D + c0) = make_float4(cb[0], cb[1], cb[2], cb[3]);
+  }
+}
+
+// at_gamma[c] += sum_b part[b][c], at_beta[c] += sum_b part[parts + b][c].  Block = 8 lanes x 32 columns: lane l adds
+// the partials b = l, l + 8, ... in order, then the lanes are added in lane order.  (One thread per column walking
+// all the partials would wait on a memory round trip per partial.)
+__global__ void __launch_bounds__(256) ln_params_finish_kernel(const float* __restrict__ part, int parts, int D,
+                                                               float* at_gamma, float* at_beta) {
+  __shared__ float red[8][32];
+  const int cl = threadIdx.x & 31, pl = threadIdx.x >> 5;
+  const int c = blockIdx.x * 32 + cl;   // 0 .. 2D-1: gamma columns, then beta columns
+  const int half = c >= D ? 1 : 0;
+  float v = 0.f;
+  if (c < 2 * D) {
+    const float* p = part + (int64_t)half * parts * D + (c - half * D);
+    for (int b = pl; b < parts; b += 8) v += p[(int64_t)b * D];
+  }
+  red[pl][cl] = v;
+  __syncthreads();
+  if (pl == 0 && c < 2 * D) {
+    float sum = red[0][cl];
 #pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      if (A.at_gamma) atomicAdd(A.at_gamma + c0 + e, cg[e]);
-      if (A.at_beta) atomicAdd(A.at_beta + c0 + e, cb[e]);
-    }
+    for (int i = 1; i < 8; ++i) sum += red[i][cl];
+    float* out = half ? at_beta : at_gamma;
+    if (out) out[c - half * D] += sum;
   }
 }
 
@@ -548,6 +577,14 @@ int bb_launch_layernorm(const bb_node& nd, int pass, cudaStream_t s) {
   A.eps = (float)nd.f[0];
   A.beta = nd.beta[0];
   if (A.rows <= 0) return BB_OK;
+  // BN_TB: per-block partials of the parameter adjoints, added in a fixed order into at_gamma / at_beta
+  auto finish_params = [&](unsigned grid) -> int {
+    if (!A.at_gamma && !A.at_beta) return BB_OK;
+    ln_params_finish_kernel<<<(unsigned)((2 * A.D + 31) / 32), 256, 0, s>>>(A.part, (int)grid, A.D, A.at_gamma, A.at_beta);
+    bb_launch_tally += 1;
+    return (int)cudaPeekAtLastError();
+  };
+  bool owned = false;
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   const bool wide = A.D % 4 == 0 && A.D >= 256 && A.D <= 1024 && al16(A.tx) && al16(A.g) && al16(A.gt) && al16(A.ty) &&
                     al16(A.gamma) && al16(A.tgamma) && al16(A.tbeta) && (reinterpret_cast<uintptr_t>(A.x) & 7) == 0 &&
@@ -565,11 +602,15 @@ int bb_launch_layernorm(const bb_node& nd, int pass, cudaStream_t s) {
       ln_row_kernel<BN_TF><<<grid, 256, 0, s>>>(A, rpb);
     } else {
       A.dst = reinterpret_cast<float*>(nd.at[0]);
+      if ((A.part = bb_partials_acquire(sizeof(float) * 2 * grid * A.D, s, &owned)) == nullptr)
+        return (int)cudaErrorMemoryAllocation;
       ln_row_kernel<BN_TB><<<grid, 256, 0, s>>>(A, rpb);
     }
     bb_launch_tally += 1;
-    BB_LAUNCH_CHECK();
-    return BB_OK;
+    int rc = (int)cudaPeekAtLastError();
+    if (rc == BB_OK && A.part) rc = finish_params(grid);
+    bb_partials_release(A.part, owned, s);
+    return rc;
   }
   const int rows_per_block = kLnWarps * kLnRowsPerWarp;
   const unsigned grid = (unsigned)((A.rows + rows_per_block - 1) / rows_per_block);
@@ -580,11 +621,18 @@ int bb_launch_layernorm(const bb_node& nd, int pass, cudaStream_t s) {
     ln_kernel<BN_TF><<<grid, kLnWarps * 32, 0, s>>>(A);
   } else {
     A.dst = reinterpret_cast<float*>(nd.at[0]);
-    const size_t smem = sizeof(float) * 2 * A.D;
-    if (smem > 48 * 1024) return BB_ERR_UNSUPPORTED;
+    const size_t smem = sizeof(float) * kLnWarps * 2 * A.D;
+    if (smem > 200 * 1024) return BB_ERR_UNSUPPORTED;
+    static BbOncePerDevice configured;
+    if (configured.need())
+      BB_CUDA_TRY(cudaFuncSetAttribute(ln_kernel<BN_TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    if ((A.part = bb_partials_acquire(sizeof(float) * 2 * grid * A.D, s, &owned)) == nullptr)
+      return (int)cudaErrorMemoryAllocation;
     ln_kernel<BN_TB><<<grid, kLnWarps * 32, smem, s>>>(A);
   }
   bb_launch_tally += 1;
-  BB_LAUNCH_CHECK();
-  return BB_OK;
+  int rc = (int)cudaPeekAtLastError();
+  if (rc == BB_OK && A.part) rc = finish_params(grid);
+  bb_partials_release(A.part, owned, s);
+  return rc;
 }

@@ -22,7 +22,7 @@ enum bb_op {
   BB_OP_LOGSOFTMAX = 13,
   BB_OP_NLL = 14,       // dims = B,C  aux[0]=int64 target  kind=reduction(0 none,1 mean,2 sum) f[0]=scale
   BB_OP_BCE_LOGITS = 15,// mean reduction               n  aux[0] = fp32 targets
-  BB_OP_EMBEDDING = 16, // dims = nidx,D,V,padding_idx  aux[0] = int64 indices
+  BB_OP_EMBEDDING = 16, // dims = nidx,D,V,padding_idx  aux[0] = int64 indices, aux[1] = sorted token positions + run ends (plan.py _n_embedding)
   BB_OP_AVGPOOL2D = 18, // linear: dims = NC,H,W,HO,WO,kh,kw,sh,sw,ph,pw  f[0] = 1/divisor
   BB_OP_CONVBLOCK = 19, // fused data-input conv3x3 -> BatchNorm -> [ReLU] -> MaxPool2d(2) (convblock.cu)
   BB_OP_CONVBLOCK2 = 20, // fused inner conv3x3 -> BatchNorm -> [ReLU] -> MaxPool2d(2) of a bf16 graph (convblock2.cu)

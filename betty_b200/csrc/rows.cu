@@ -141,14 +141,39 @@ __global__ void emb_fwd_kernel(const float* __restrict__ tw, const int64_t* __re
   ty[i] = tw[idx[r] * D + (i - r * D)];
 }
 
-__global__ void emb_bwd_kernel(float* gw, const int64_t* __restrict__ idx, const float* __restrict__ gy, int64_t nidx,
-                               int D, int64_t padding_idx) {
-  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nidx * D) return;
-  const int64_t r = i / D;
-  const int64_t row = idx[r];
-  if (row == padding_idx) return;
-  atomicAdd(gw + row * D + (i - r * D), gy[i]);
+// gw[row] += sum of gy over the tokens that gathered row, in a fixed order.  seg[0..nidx) = the token positions stably
+// sorted by table row, seg[nidx + j] = end of the row's run in that order if j starts one, else 0 (built with the plan).
+// Block = 16 token lanes x 32 columns, walking the runs that start at j = blockIdx.y, +gridDim.y, ...: lane l adds the
+// run's tokens l, l + 16, ... in order, then the lanes are added in lane order (a row every token shares, such as the
+// token-type row, is one run of all nidx tokens).
+constexpr int kEmbLanes = 16;
+__global__ void __launch_bounds__(kEmbLanes * 32) emb_bwd_kernel(float* gw, const int64_t* __restrict__ idx,
+                                                                 const int64_t* __restrict__ seg,
+                                                                 const float* __restrict__ gy, int64_t nidx, int D,
+                                                                 int64_t padding_idx) {
+  __shared__ float red[kEmbLanes][32];
+  const int cl = threadIdx.x & 31, tl = threadIdx.x >> 5;
+  const int64_t col = (int64_t)blockIdx.x * 32 + cl;
+  for (int64_t j = blockIdx.y; j < nidx; j += gridDim.y) {
+    const int64_t end = seg[nidx + j];
+    if (end == 0) continue;   // uniform over the block
+    const int64_t row = idx[seg[j]];
+    if (row == padding_idx) continue;
+    float v = 0.f;
+    if (col < D) {
+#pragma unroll 4
+      for (int64_t k = j + tl; k < end; k += kEmbLanes) v += gy[seg[k] * D + col];
+    }
+    red[tl][cl] = v;
+    __syncthreads();
+    if (tl == 0 && col < D) {
+      float sum = red[0][cl];
+#pragma unroll
+      for (int i = 1; i < kEmbLanes; ++i) sum += red[i][cl];
+      gw[row * D + col] += sum;
+    }
+    __syncthreads();
+  }
 }
 
 // ---- max-pool: gather / scatter with the base argmax ---------------------------------------------------
@@ -332,8 +357,11 @@ int bb_launch_embedding(const bb_node& nd, int pass, cudaStream_t s) {
     emb_fwd_kernel<<<blocks(nidx * D, 256), 256, 0, s>>>(reinterpret_cast<const float*>(nd.t[0]), idx,
                                                          reinterpret_cast<float*>(nd.t[3]), nidx, D);
   } else if (pass == BB_PASS_TAN_BWD) {
-    emb_bwd_kernel<<<blocks(nidx * D, 256), 256, 0, s>>>(reinterpret_cast<float*>(nd.at[0]), idx,
-                                                         reinterpret_cast<const float*>(nd.at[3]), nidx, D, nd.dims[3]);
+    const int64_t* seg = reinterpret_cast<const int64_t*>(nd.aux[1]);
+    if (seg == nullptr) return BB_ERR_ARG;
+    const dim3 grid((unsigned)((D + 31) / 32), (unsigned)(nidx < 128 ? nidx : 128));
+    emb_bwd_kernel<<<grid, kEmbLanes * 32, 0, s>>>(reinterpret_cast<float*>(nd.at[0]), idx, seg,
+                                                   reinterpret_cast<const float*>(nd.at[3]), nidx, D, nd.dims[3]);
   } else {
     return BB_OK;  // base adjoint of a parameter table is never needed
   }

@@ -50,6 +50,10 @@ int bb_partials_reduce(const float* part, int parts, int64_t n, float* out, cuda
 // stream-ordered allocation released by bb_partials_release (launches outside a plan, e.g. the C-ABI unit hooks).
 float* bb_partials_acquire(size_t bytes, cudaStream_t s, bool* owned);
 void bb_partials_release(float* p, bool owned, cudaStream_t s);
+// Second half of a split-K product (gemm_tma.cu, gemm_tc.cu): out[m*ors + n*ocs] (beta)= bias[n*bias_stride] + the
+// ksplit partials part[sp][m][n] (col_major: part[sp][n][m]) added in split order.
+int bb_splitk_finish(const float* part, int ksplit, int64_t M, int64_t N, bool col_major, float* out, int64_t ors,
+                     int64_t ocs, int beta, const float* bias, int64_t bias_stride, cudaStream_t s);
 
 // Per-node buffer that lives as long as the plan, for packs of operands that are constant across the K-loop (the
 // im2col matrix of a data-input convolution).  Returns nullptr when the plan has no persistent arena (or it is full);

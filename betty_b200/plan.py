@@ -567,6 +567,18 @@ class HvpPlan:
         pad = n.attrs["padding_idx"]
         r["dims"][0:4] = (idx.numel(), D, V, -1 if pad is None else pad)
         r["aux"][0] = self._const(idx, torch.int64).data_ptr()
+        # the token positions stably sorted by table row, then for each sorted position the end of the row's run if
+        # one starts there (else 0): the backward adds each row's tokens in a fixed order without atomics
+        def runs(src=idx):
+            ids, order = torch.sort(src.detach().reshape(-1).to(torch.int64), stable=True)
+            n = ids.numel()
+            starts = torch.ones(n, dtype=torch.bool, device=ids.device)
+            starts[1:] = ids[1:] != ids[:-1]
+            first = torch.nonzero(starts).reshape(-1)
+            ends = torch.zeros(n, dtype=torch.int64, device=ids.device)
+            ends[first] = torch.cat([first[1:], first.new_tensor([n])])
+            return torch.cat([order, ends])
+        r["aux"][1] = self._const(runs(), torch.int64, recipe=runs).data_ptr()
         if not n.out.base.is_contiguous():
             raise UnsupportedGraph("embedding output must be contiguous")
         self._slot(r, 0, w, w.base)

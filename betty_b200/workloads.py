@@ -321,9 +321,10 @@ def fourconv_imaml(device="cpu", method="neumann", n=25, ways=5, image="omniglot
 
 
 def roberta_reweight(device="cpu", method="cg", batch=16, seq=50, K=10, alpha=1.0, l2=5e-3, precision="fp32",
-                     tiny=False, tiny_hidden=32, seed=0):
+                     tiny=False, tiny_hidden=32, seed=0, layers=12):
     """Config 5: HF RobertaForSequenceClassification (random init, eager attention, dropout 0) with
-    MWN-weighted CE (reference examples/bert_data_reweighting/main.py:117-128, model.py:11-59)."""
+    MWN-weighted CE (reference examples/bert_data_reweighting/main.py:117-128, model.py:11-59).  ``layers`` shortens
+    the RoBERTa-base encoder (12 layers) for tests whose float64 reference would not fit in memory at full depth."""
     from transformers import RobertaConfig, RobertaForSequenceClassification
 
     torch.manual_seed(seed)
@@ -332,7 +333,7 @@ def roberta_reweight(device="cpu", method="cg", batch=16, seq=50, K=10, alpha=1.
                            intermediate_size=2 * tiny_hidden, max_position_embeddings=seq + 4, num_labels=2,
                            hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0)
     else:
-        hc = RobertaConfig(vocab_size=50265, hidden_size=768, num_hidden_layers=12, num_attention_heads=12,
+        hc = RobertaConfig(vocab_size=50265, hidden_size=768, num_hidden_layers=layers, num_attention_heads=12,
                            intermediate_size=3072, max_position_embeddings=514, type_vocab_size=1,
                            num_labels=2, hidden_dropout_prob=0.0, attention_probs_dropout_prob=0.0)
     hc._attn_implementation = "eager"
@@ -347,7 +348,8 @@ def roberta_reweight(device="cpu", method="cg", batch=16, seq=50, K=10, alpha=1.
     cfg = ShimConfig(type=method, precision=precision, neumann_iterations=K, neumann_alpha=alpha,
                      cg_iterations=K, cg_alpha=alpha)
     return _pair("bert_data_reweighting", lower, _roberta_reweight_step(l2), upper, cfg, (ids, mask, seg, y),
-                 device, describe=dict(batch=batch, seq=seq, K=K, method=method, precision=precision, tiny=tiny))
+                 device, describe=dict(batch=batch, seq=seq, K=K, method=method, precision=precision, tiny=tiny,
+                                       **({} if tiny or layers == 12 else dict(layers=layers))))
 
 
 # -- config 4: a compact DARTS-style supernet (mixed ops weighted by softmax(alpha)) --------------

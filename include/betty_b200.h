@@ -168,6 +168,19 @@ int bb_gemm_bf16_tma(int64_t M, int64_t N, int64_t K, const void* A, int dtA, in
                      int dtB, int64_t brs, int64_t bcs, float* C, int64_t crs, int64_t ccs, int beta, void* scratch,
                      int64_t scratch_bytes, void* stream);
 
+/* every option of the TMA-fed product, for unit tests: npairs (1-2) operand pairs summed into one output,
+ *   C[b][m][n] (beta)= sum_p sum_k A_p[b][m][k] B_p[b][k][n] (+ bias[n*bias_stride]),
+ * A_p[b][m][k] = A[p][b*a_desc[4p+3] + m*a_desc[4p+1] + k*a_desc[4p+2]] with dtype a_desc[4p] (B likewise:
+ * b_desc[4p..4p+3] = dt, brs, bcs, bbs), C[b][m][n] = C[b*cbs + m*crs + n*ccs], or the NCHW plane layout
+ * C[(img*N + n)*plane_ohw + q] for m = img*plane_ohw + q when plane_ohw > 0.  flags force the tile width (1: 64,
+ * 2: 128), turn the persistent kernel off (4) or force a split-K count (n << 8).  route (7 ints) receives the
+ * configuration launched: bn, ksplit, persistent, then the operand layouts of A_0, B_0, A_1, B_1 (0 k-major,
+ * 1 m/n-major, -1 absent).  Returns 1 if the launcher declines the job. */
+int bb_gemm_bf16_tma_ex(int64_t M, int64_t N, int64_t K, int npairs, int64_t batch, const void* const* A,
+                        const int64_t* a_desc, const void* const* B, const int64_t* b_desc, float* C, int64_t crs,
+                        int64_t ccs, int64_t cbs, int beta, const float* bias, int64_t bias_stride, int plane_ohw,
+                        int min_n, int flags, void* scratch, int64_t scratch_bytes, int* route, void* stream);
+
 const char* bb_version(void);
 
 #ifdef __cplusplus
