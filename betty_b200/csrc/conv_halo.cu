@@ -14,9 +14,11 @@
 // loaded once per CTA and stay resident.  Shared-memory fill per tile: 2 x 28 KB instead of 2 x 9 x 24 KB.  Rows that
 // fall on the zero border compute garbage-free zeros' neighbours and are simply not stored.
 //
-// Roles (288 threads, one CTA per SM, persistent over tiles): warps 0-7 = two consumer warpgroups (rows 64g..64g+63
-// of a tile, register accumulators, epilogue -> fp32 NCHW planes or bf16 padded NHWC), warp 8 = TMA producer.  Up to
-// four band buffers are in flight, so the next tiles' loads overlap a tile's epilogue.
+// Roles (288 threads, one CTA per SM, persistent over tiles): warps 0-7 = two consumer warpgroups (register
+// accumulators, epilogue -> bf16 padded NHWC or fp32 NCHW planes), warp 8 = TMA producer.  With bf16 output the
+// warpgroups take the CTA's tiles in turn, all 128 rows each, so that one issues a tile's wgmma while the other drains
+// its tile and runs the epilogue; with fp32 output both work on every tile, 64 rows each.  Up to four band buffers are
+// in flight.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include <string.h>
@@ -40,7 +42,10 @@ constexpr int BAND_ROWS = 256;                 // TMA box limit; a band needs 12
 constexpr int BAND_BYTES = BAND_ROWS * 128;    // 32 KB
 constexpr int W_TILE = 64 * 128;               // one tap's weights: 64 rows (n) x 64 ch
 constexpr int MAXBAND = 4;                     // activation bands in flight: 4 with one operand pair, 2 with two
-constexpr int STG_BYTES = 64 * 128;            // one warpgroup's 64 output rows in bf16
+constexpr uint32_t HALF16 = 64 * 128 / 16;     // rows 64-127 of a tile: 64 band rows further, in 16-byte units
+constexpr int STG_BYTES = 64 * 128;            // 64 output rows in bf16: one warpgroup's staging, used per tile half
+constexpr int STG_BAR = 1, TURN_BAR = 3;       // named barriers: 1, 2 = staging of warpgroup 0, 1; 3, 4 = issue turn of
+                                               // warpgroup 0, 1; 5 = end of the phase-timing run
 
 struct alignas(64) HaloArgs {
   CUtensorMap a[2];          // padded activation as a matrix [rows][64] (rank-3 map, batch 1), box (64, band_rows)
@@ -63,13 +68,13 @@ struct alignas(64) HaloArgs {
   int phase_slots;              // tile slots per CTA in `phases` (tiles per CTA + 1)
 };
 
-// Phase timing (conv_halo_kernel<..., PHASES = true>, reached only through bb_conv_halo_phases): thread 0 of each
-// consumer warpgroup writes clock64() at the points named by PHASE_NAMES, in program order, into
+// Phase timing (conv_halo_kernel<..., PHASES = true>, reached only through bb_conv_halo_phases): thread 0 of the
+// consumer warpgroup that owns a tile writes clock64() at the points named by PHASE_NAMES, in program order, into
 //   phases[4 * grid + ((cta * phase_slots + slot) * 2 + wg) * NSTAMP + k]
 // and thread 0 of the CTA writes {globaltimer, clock64} at the start and the end of its tile loop into phases[4 * cta ...]
-// (so the SM clock can be recovered).  A point that a schedule does not pass stays 0.
+// (so the SM clock can be recovered).  Slot = the CTA's local tile index; wg = slot & 1, the other entry stays 0.
 constexpr int NSTAMP = 8;
-constexpr const char* PHASE_NAMES = "top,p0_band,last_band,issued,drained,epilogue";
+constexpr const char* PHASE_NAMES = "top,turn,p0_band,last_band,issued,drained,epilogue";
 
 __device__ __forceinline__ uint64_t globaltimer() {
   uint64_t v;
@@ -79,7 +84,8 @@ __device__ __forceinline__ uint64_t globaltimer() {
 
 
 // Shared memory: [npairs x 9 x 8 KB] weights (resident for the whole kernel) | [NB x band_alloc] activation bands |
-// [2 x 8 KB] bf16 output staging, one 64-row block per consumer warpgroup (BF16OUT only) | barriers.  The MMA issue loop stays free of waits: both pairs' weights are resident rather than streamed through a
+// [2 x 8 KB] bf16 output staging, one 64-row block per consumer warpgroup, filled and copied out once per tile half
+// (BF16OUT only) | barriers.  The MMA issue loop stays free of waits: both pairs' weights are resident rather than streamed through a
 // ring with a wait per tap, and two bands are in flight.
 template <int NB, bool BF16OUT, bool PHASES>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_constant__ HaloArgs G) {
@@ -97,7 +103,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
     mbar_init(wfull, 1);
     for (int b = 0; b < MAXBAND; ++b) {
       mbar_init(bfull0 + 8 * b, 1);
-      mbar_init(bempty0 + 8 * b, 2);   // one arrival per consumer warpgroup
+      mbar_init(bempty0 + 8 * b, BF16OUT ? 1 : 2);   // consumer warpgroups that read each band
     }
     fence_barrier_init();
   }
@@ -137,24 +143,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
   for (int q = 0; q < 9; ++q) {
     const int i = q / 3, j = q - 3 * i;
     const int dy = G.flip ? 1 - i : i - 1, dx = G.flip ? 1 - j : j - 1;
-    tap16[q] = (uint32_t)((G.Wp + 1 + dy * G.Wp + dx + wg * 64) * 8);
+    tap16[q] = (uint32_t)((G.Wp + 1 + dy * G.Wp + dx) * 8);
   }
   const uint32_t w16 = (smem_u32(wsm) & 0x3FFFF) >> 4, band16_0 = (smem_u32(bands) & 0x3FFFF) >> 4;
   const uint32_t band16_step = (uint32_t)G.band_alloc >> 4;
   const int64_t HW = (int64_t)G.H * G.W;
-  // Epilogue without divisions: each thread's output rows are a fixed offset rb into the tile plus steps of ST rows
+  // Epilogue without divisions: each thread's output rows are a fixed offset rb into the tile half plus steps of ST rows
   // (bf16 copy-out: rows t/8 + 16 it; fp32 NCHW: rows frag_row + 8 h).  The first row's (image, y, x) is found once
-  // per tile and the next ones by adding the step's precomputed (dy, dx) with a carry.
+  // per half and the next ones by adding the step's precomputed (dy, dx) with a carry.
   constexpr int ST = BF16OUT ? 16 : 8;
-  const int rb = wg * 64 + (BF16OUT ? (t >> 3) : frag_row(t));
+  const int rb = BF16OUT ? (t >> 3) : frag_row(t);
   const int Hp = G.HpWp / G.Wp, sy = ST / G.Wp, sx = ST - sy * G.Wp;
   // this thread's 16 output channels' bias, read once
   const bool has_bias = G.bias != nullptr;
+  // (bf16 output, transposed product: channels frag_row and frag_row + 8; fp32 output: channels 8 j + frag_col + e)
   float bz[BN / 4];
+  if constexpr (BF16OUT) {
+    bz[0] = has_bias ? G.bias[frag_row(t)] : 0.f;
+    bz[1] = has_bias ? G.bias[frag_row(t) + 8] : 0.f;
+  } else {
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j)
+    for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-    for (int e = 0; e < 2; ++e) bz[2 * j + e] = has_bias ? G.bias[8 * j + frag_col(t) + e] : 0.f;
+      for (int e = 0; e < 2; ++e) bz[2 * j + e] = has_bias ? G.bias[8 * j + frag_col(t) + e] : 0.f;
+  }
   mbar_wait(wfull, 0);
   unsigned long long* ph = nullptr;
   if constexpr (PHASES) {
@@ -166,8 +178,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
   };
 
   // ---------------- epilogue: d[4j + 2h + e] = (row frag_row + 8h, channel 8j + frag_col + e) ----------------
-  auto epilogue = [&](float (&a)[BN / 2], int tile) {
-    int row = tile * BM + rb;   // padded-linear pixel index of this thread's first row
+  auto epilogue = [&](auto& a, int tile, int half) {
+    int row = tile * BM + half * 64 + rb;   // padded-linear pixel index of this thread's first row
     int img = (int)((unsigned)row / (unsigned)G.HpWp);
     int yy = row - img * G.HpWp;
     int xx = yy;
@@ -179,22 +191,32 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
       if (yy >= Hp) { yy -= Hp; ++img; }
     };
     if constexpr (BF16OUT) {
-      // bf16 padded-NHWC output: this warpgroup's 64 rows are one contiguous 8 KB block of the output.  Stored from the
-      // fragments, each warp store would cover eight half sectors; staged in shared memory (16-byte chunk j of row r at
-      // r*128 + 16 (j ^ (r & 7)), free of bank conflicts) it goes out as whole 16-byte chunks, border rows as zeros.
+      // bf16 padded-NHWC output: the half's 64 rows are one contiguous 8 KB block of the output.  The accumulator is
+      // the transposed tile (row = channel, column = pixel); stmatrix.trans writes its 8x8 blocks back as pixel rows
+      // into shared memory (16-byte chunk c of row r at r*128 + 16 (c ^ (r & 7)), free of bank conflicts), and the
+      // block goes out as whole 16-byte chunks, border rows as zeros.
       uint8_t* st = stg + wg * STG_BYTES;
-      named_barrier_sync(1 + wg, 128);    // per warpgroup; the previous tile's copy-out has read the staging block
+      named_barrier_sync(STG_BAR + wg, 128);    // the previous half's copy-out has read the staging block
+      {
+        // block q of the x4 = (pixels 8 (j + q/2) .. + 7 of the half, channels 16 warp + 8 (q & 1) .. + 7); lane L
+        // addresses the pixel row L % 8 of block L / 8
+        const int lane = t & 31, blk = lane >> 3, chunk = 2 * (t >> 5) + (blk & 1);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int r = frag_row(t) + 8 * h;
+        for (int j = 0; j < 8; j += 2) {
+          uint32_t v[4];
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          float f0 = a[4 * j + 2 * h], f1 = a[4 * j + 2 * h + 1];
-          if (has_bias) { f0 += bz[2 * j]; f1 += bz[2 * j + 1]; }
-          *reinterpret_cast<__nv_bfloat162*>(st + r * 128 + 16 * (j ^ (r & 7)) + 2 * frag_col(t)) = __floats2bfloat162_rn(f0, f1);
+          for (int q = 0; q < 4; ++q) {
+            const int jj = 8 * half + j + (q >> 1), h = q & 1;
+            float f0 = a[4 * jj + 2 * h], f1 = a[4 * jj + 2 * h + 1];
+            if (has_bias) { f0 += bz[h]; f1 += bz[h]; }
+            const __nv_bfloat162 b2 = __floats2bfloat162_rn(f0, f1);
+            v[q] = *reinterpret_cast<const uint32_t*>(&b2);
+          }
+          const int r = 8 * (j + (blk >> 1)) + (lane & 7);
+          stmatrix_x4_trans(smem_u32(st) + (uint32_t)(r * 128 + 16 * (chunk ^ (r & 7))), v[0], v[1], v[2], v[3]);
         }
       }
-      named_barrier_sync(1 + wg, 128);
+      named_barrier_sync(STG_BAR + wg, 128);
 #pragma unroll
       for (int it = 0; it < 4; ++it) {
         const int r = (t >> 3) + 16 * it, c = t & 7;
@@ -227,41 +249,77 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_halo_kernel(const __grid_con
     }
   };
 
-  float acc[BN / 2];
-  int git = 0, lt = 0;
-  for (int tile = blockIdx.x; tile < G.ntiles; tile += gridDim.x, ++lt) {
+  // bf16 output -- ping-pong over whole tiles: local tile lt of this CTA belongs to warpgroup lt & 1, which accumulates
+  // all 128 rows.  Issue is ordered: a warpgroup starts tile lt once the other
+  // one has committed the last wgmma of tile lt - 1, so the tensor pipe has one warpgroup's work queued while the other
+  // drains and runs its epilogue.  A warpgroup arrives on the other's turn barrier only when a next tile exists, so every
+  // arrival meets exactly one wait (0 or 1 tiles: no barrier at all; odd or even counts: each tile lt >= 1 waits once,
+  // on the arrival its predecessor made).
+  // fp32 NCHW output -- both warpgroups take every tile, rows 64 wg .. 64 wg + 63: that epilogue is a strided
+  // read-modify-write bound by memory, which gains more from both warpgroups writing at once than from overlapping it
+  // with the MMA (tools/halo_bench.py, DESIGN section 7).
+  // The ping-pong warpgroup computes the tile transposed, out^T[channel][pixel] = W . band^T, as one wgmma m64n128k16
+  // per k-step with the weights as A and the 128 band rows as B: 6 KB of shared-memory operands per step where two
+  // m64n64k16 over the two 64-row halves read 8 KB.  Per element the sum runs over the same products in the same order.
+  constexpr bool PP = BF16OUT;
+  const uint32_t row16 = PP ? 0u : (uint32_t)wg * HALF16;
+  const int my_tiles = (int)blockIdx.x < G.ntiles ? (G.ntiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  float acc[PP ? BN : BN / 2];
+  auto fence_all = [&]() { fence_acc(acc); };
+  for (int lt = PP ? wg : 0; lt < my_tiles; lt += PP ? 2 : 1) {
+    const int tile = (int)blockIdx.x + lt * (int)gridDim.x;
     stamp(lt, 0);
+    if (PP && lt > 0) named_barrier_sync(TURN_BAR + wg, 256);
+    stamp(lt, 1);
+    int git = lt * G.npairs;
     for (int p = 0; p < G.npairs; ++p, ++git) {
       const int b = git % NB;
       mbar_wait(bfull0 + 8 * b, (git / NB) & 1);
-      if (p == 0) stamp(lt, 1);
-      if (p == G.npairs - 1) stamp(lt, 2);
-      const uint32_t band16 = band16_0 + (uint32_t)b * band16_step;
+      if (p == 0) stamp(lt, 2);
+      if (p == G.npairs - 1) stamp(lt, 3);
+      const uint32_t band16 = band16_0 + (uint32_t)b * band16_step + row16;
       const uint32_t wp16 = w16 + (uint32_t)p * (9 * W_TILE >> 4);
-      fence_acc(acc);
+      fence_all();
       wgmma_fence();
 #pragma unroll
       for (int q = 0; q < 9; ++q) {
         const uint32_t alo = band16 + tap16[q], blo = wp16 + (uint32_t)q * (W_TILE >> 4);
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-          wgmma_n64<0, 0>(acc, dhi | (uint64_t)(alo + 2 * k), dhi | (uint64_t)(blo + 2 * k), (p > 0 || q > 0 || k > 0) ? 1u : 0u);
+        for (int k = 0; k < 4; ++k) {
+          const uint32_t sc = (p > 0 || q > 0 || k > 0) ? 1u : 0u;
+          if constexpr (PP)
+            wgmma_n128<0, 0>(acc, dhi | (uint64_t)(blo + 2 * k), dhi | (uint64_t)(alo + 2 * k), sc);
+          else
+            wgmma_n64<0, 0>(acc, dhi | (uint64_t)(alo + 2 * k), dhi | (uint64_t)(blo + 2 * k), sc);
+        }
+        if (q == 0) {
+          // tap 0 is a group of its own: once the group before it (the previous pair) completes, that pair's band is
+          // released and the producer reloads it while this pair's remaining eight taps are issued
+          wgmma_commit();
+          fence_all();
+          wgmma_wait<1>();
+          if (p > 0 && t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
+        }
       }
       wgmma_commit();
-      if (p == G.npairs - 1) stamp(lt, 3);
-      fence_acc(acc);
-      wgmma_wait<1>();
-      if (p > 0 && t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
     }
-    wgmma_wait<0>();
-    fence_acc(acc);
     stamp(lt, 4);
-    if (t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
-    epilogue(acc, tile);
+    if (PP && lt + 1 < my_tiles) named_barrier_arrive(TURN_BAR + (wg ^ 1), 256);
+    fence_all();
+    wgmma_wait<0>();
+    fence_all();
     stamp(lt, 5);
+    if (t == 0) mbar_arrive(bempty0 + 8 * ((git - 1) % NB));
+    if constexpr (PP) {
+      epilogue(acc, tile, 0);
+      epilogue(acc, tile, 1);
+    } else {
+      epilogue(acc, tile, wg);
+    }
+    stamp(lt, 6);
   }
   if constexpr (PHASES) {
-    named_barrier_sync(3, 256);   // ids 1 and 2 are the warpgroups' epilogue barriers
+    named_barrier_sync(TURN_BAR + 2, 256);
     if (tid == 0) { G.phases[4 * blockIdx.x + 2] = globaltimer(); G.phases[4 * blockIdx.x + 3] = clock64(); }
   }
 }

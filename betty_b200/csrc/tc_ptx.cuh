@@ -149,6 +149,18 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint6
 __device__ __forceinline__ void named_barrier_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
 }
+// arrive on hardware barrier `id` without waiting; the barrier completes when `count` threads have arrived or synced
+__device__ __forceinline__ void named_barrier_arrive(int id, int count) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// four 8x8 b16 matrices to shared memory, each transposed: register q holds this lane's two elements (row lane / 4,
+// columns 2 (lane % 4), +1) of matrix q, and the address lane L gives receives column L % 8 of matrix L / 8
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
 
 // Accumulator fragment of m64nN for thread t of the warpgroup: d[4j + 2h + e] holds row 16*(t/32) + (t%32)/4 + 8h,
 // column 8j + 2*(t%4) + e.

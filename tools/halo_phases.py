@@ -2,12 +2,14 @@
 42x42, 21x21 and 10x10), with two operand pairs and with one.
 
 A separate instantiation of the kernel (bb_conv_halo_phases; the plan and the K-loop never launch it) has thread 0 of
-each consumer warpgroup read clock64() at fixed points of its tile loop.  The library names the points
-(bb_conv_halo_phase_names) in program order; each phase below is the time from one recorded point to the next one of
-the same tile slot, and `period` is the time from one tile slot's first point to the next one's, i.e. the cost of a
-tile.  Cycles become nanoseconds at the SM clock the same run shows (clock64 over globaltimer, per CTA).  The first
-tile slot of each CTA is left out (it waits for the resident weights).  The stamps cost a few instructions per point,
-so the phase variant runs slightly slower than the default one; compare it with itself across builds.
+the consumer warpgroup that owns a tile (local tile lt of a CTA -> warpgroup lt & 1) read clock64() at fixed points of
+its tile loop.  The library names the points (bb_conv_halo_phase_names) in program order; each phase below is the time
+from one recorded point to the next one of the same tile, per warpgroup: the wait for the issue turn (top -> turn), the
+band waits, the issue, the drain and the epilogue.  `period` is the time from one tile's `turn` (its first wgmma) to
+the next tile's, i.e. the cost of a tile to the tensor pipe.  Cycles become nanoseconds at the SM clock the same run
+shows (clock64 over globaltimer, per CTA).  Each warpgroup's first tile is left out (it waits for the resident
+weights).  The stamps cost a few instructions per point, so the phase variant runs slightly slower than the default
+one; compare it with itself across builds.
 With BB200_LIB=<path> the same run measures another build of the library.
     python tools/halo_phases.py [N H W] [--reps R]"""
 import argparse
@@ -71,6 +73,7 @@ def measure(n, h, w, npairs, reps):
 def summarize(grid, slots, nst, samples, names):
     phases, periods, ghz, kernel_us = {}, [], [], []
     order = []
+    turn = names.index("turn")
     for s in samples:
         hdr = s[:4 * grid].reshape(grid, 4)
         ratio = (hdr[:, 3] - hdr[:, 1]) / np.maximum(hdr[:, 2] - hdr[:, 0], 1)   # cycles per ns
@@ -79,24 +82,22 @@ def summarize(grid, slots, nst, samples, names):
         cyc_ns = np.median(ratio)
         v = s[4 * grid:].reshape(grid, slots, 2, nst)
         for c in range(grid):
-            for wg in range(2):
-                prev_top = None
-                for sl in range(slots):
-                    row = v[c, sl, wg]
-                    ks = [k for k in range(nst) if row[k] != 0]
-                    if not ks:
-                        continue
-                    if sl > 0:
-                        for a, b in zip(ks, ks[1:]):
-                            key = f"{names[a]} -> {names[b]}"
-                            if key not in phases:
-                                phases[key] = []
-                                order.append(key)
-                            phases[key].append((row[b] - row[a]) / cyc_ns)
-                    if row[0] != 0:
-                        if prev_top is not None and sl > 1:
-                            periods.append((row[0] - prev_top) / cyc_ns)
-                        prev_top = row[0]
+            prev_turn = None
+            for sl in range(slots):
+                wg = sl & 1
+                row = v[c, sl, wg]
+                ks = [k for k in range(nst) if row[k] != 0]
+                if not ks:
+                    continue
+                if sl > 1:
+                    for a, b in zip(ks, ks[1:]):
+                        key = f"{names[a]} -> {names[b]}"
+                        if key not in phases:
+                            phases[key] = ([], [])
+                            order.append(key)
+                        phases[key][wg].append((row[b] - row[a]) / cyc_ns)
+                    periods.append((row[turn] - prev_turn) / cyc_ns)
+                prev_turn = row[turn]
     return order, phases, periods, float(np.median(ghz)), float(np.median(kernel_us))
 
 
@@ -117,12 +118,15 @@ def main():
             order, phases, periods, ghz, kus = summarize(grid, slots, nst, samples, names)
             print(f"\nN={n} {h}x{w}, {npairs} pair{'s' if npairs > 1 else ''}: {grid} CTAs, up to {slots - 1} tiles each, "
                   f"phase kernel {kus:.1f} us, SM clock {ghz * 1e3:.0f} MHz")
-            print(f"  {'phase':34s} {'median ns':>10s} {'p90 ns':>10s}")
+            print(f"  {'phase':34s} {'wg0 median':>10s} {'p90':>7s} {'wg1 median':>10s} {'p90':>7s}   (ns)")
             for key in order:
-                x = np.asarray(phases[key])
-                print(f"  {key:34s} {np.median(x):10.0f} {np.percentile(x, 90):10.0f}")
+                cols = []
+                for x in phases[key]:
+                    cols += [np.median(x), np.percentile(x, 90)] if x else [np.nan, np.nan]
+                print(f"  {key:34s} {cols[0]:10.0f} {cols[1]:7.0f} {cols[2]:10.0f} {cols[3]:7.0f}")
             x = np.asarray(periods)
-            print(f"  {'period (tile to tile)':34s} {np.median(x):10.0f} {np.percentile(x, 90):10.0f}")
+            if x.size:
+                print(f"  {'period (turn to next turn)':34s} {np.median(x):10.0f} {np.percentile(x, 90):7.0f}")
 
 
 if __name__ == "__main__":
