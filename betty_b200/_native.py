@@ -70,6 +70,7 @@ _SIGS = {
     "bb_plan_invalidate_constants": ([C.c_void_p], 0),
     "bb_plan_graph_captures": ([C.c_void_p], 0),
     "bb_plan_node_route": ([C.c_void_p, C.c_int, C.c_int], 0),
+    "bb_conv_small_geometry": ([C.c_int] * 11 + [C.c_void_p, C.c_int], 0),
     "bb_conv_halo_bf16": ([C.c_int] * 4 + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p], 1),
     "bb_conv_halo_bf16_nhwc": ([C.c_int] * 4 + [C.c_void_p] * 4 + [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p], 1),
     "bb_conv_halo_phases": ([C.c_int] * 4 + [C.c_void_p] * 4 + [C.c_int] + [C.c_void_p] * 5, None),

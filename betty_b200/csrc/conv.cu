@@ -214,6 +214,23 @@ TcSrc wdgrad(const void* p, int dt, const Geom& g) {
   return s;
 }
 
+// the small-channel kernels' view of a stride-1 node: its own geometry (tangent forward and weight gradient), and the
+// data gradient as a correlation with the transposed, flipped weights over the output-side maps; launchers add pointers
+SmallConvArgs small_fwd_args(const Geom& g) {
+  SmallConvArgs A{};
+  A.mode = 0;
+  A.N = g.N; A.CI = g.C; A.H = g.H; A.W = g.W; A.CO = g.O; A.KH = g.KH; A.KW = g.KW; A.HO = g.HO; A.WO = g.WO;
+  A.ph = g.ph; A.pw = g.pw; A.C_orig = g.C;
+  return A;
+}
+SmallConvArgs small_dgrad_args(const Geom& g) {
+  SmallConvArgs A{};
+  A.mode = 1;
+  A.N = g.N; A.CI = g.O; A.H = g.HO; A.W = g.WO; A.CO = g.C; A.KH = g.KH; A.KW = g.KW; A.HO = g.H; A.WO = g.W;
+  A.ph = g.KH - 1 - g.ph; A.pw = g.KW - 1 - g.pw; A.C_orig = g.C;
+  return A;
+}
+
 // second-generation small-channel kernels first (conv_small2.cu), the first generation when they decline
 int small_corr(const SmallConvArgs& A, cudaStream_t s) {
   if (!getenv("BB200_CONV_SMALL_V1")) {
@@ -270,16 +287,14 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     return bb_gemm_tc_run(G, s);
   }
   if (pass == BB_PASS_TAN_FWD && unit && bb_conv_small_corr_ok(g.C, g.O, g.KH, g.KW, (actX ? 1 : 0) + (actW ? 1 : 0))) {
-    SmallConvArgs A{};
+    SmallConvArgs A = small_fwd_args(g);
     int np = 0;
     if (actX) { A.in[np] = nd.t[0]; A.dt_in[np] = BB_F32; A.w[np] = nd.base[1]; A.dt_w[np] = nd.dt[1]; ++np; }
     if (actW) { A.in[np] = nd.base[0]; A.dt_in[np] = nd.dt[0]; A.w[np] = nd.t[1]; A.dt_w[np] = BB_F32; ++np; }
-    A.npairs = np; A.mode = 0;
+    A.npairs = np;
     A.out = reinterpret_cast<float*>(nd.t[3]);
     A.bias = actB ? reinterpret_cast<const float*>(nd.t[2]) : nullptr;
     A.beta = 0;
-    A.N = g.N; A.CI = g.C; A.H = g.H; A.W = g.W; A.CO = g.O; A.KH = g.KH; A.KW = g.KW; A.HO = g.HO; A.WO = g.WO;
-    A.ph = g.ph; A.pw = g.pw; A.C_orig = g.C;
     return small_corr(A, s);
   }
   if (pass == BB_PASS_TAN_FWD) {
@@ -310,16 +325,14 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     rc = bb_gemm_tc_run(G, s);
     if (rc) return rc;
   } else if ((need & 1) && unit && bb_conv_small_corr_ok(g.O, g.C, g.KH, g.KW, (!base && actW) ? 2 : 1)) {
-    SmallConvArgs A{};
+    SmallConvArgs A = small_dgrad_args(g);
     int np = 0;
     A.in[np] = gy; A.dt_in[np] = BB_F32; A.w[np] = nd.base[1]; A.dt_w[np] = nd.dt[1]; ++np;
     if (!base && actW) { A.in[np] = nd.a[3]; A.dt_in[np] = BB_F32; A.w[np] = nd.t[1]; A.dt_w[np] = BB_F32; ++np; }
-    A.npairs = np; A.mode = 1;
+    A.npairs = np;
     A.out = reinterpret_cast<float*>(base ? nd.a[0] : nd.at[0]);
     A.bias = nullptr;
     A.beta = nd.beta[0];
-    A.N = g.N; A.CI = g.O; A.H = g.HO; A.W = g.WO; A.CO = g.C; A.KH = g.KH; A.KW = g.KW; A.HO = g.H; A.WO = g.W;
-    A.ph = g.KH - 1 - g.ph; A.pw = g.KW - 1 - g.pw; A.C_orig = g.C;
     rc = small_corr(A, s);
     if (rc) return rc;
   } else if (need & 1) {
@@ -351,7 +364,7 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     rc = bb_gemm_tc_run(G, s);
     if (rc) return rc;
   } else if ((need & 2) && unit && bb_conv_small_wgrad_ok(g.O, g.C, g.H, g.W, g.HO, g.WO, g.KH, g.KW)) {
-    SmallConvArgs A{};
+    SmallConvArgs A = small_fwd_args(g);
     int np = 0;
     A.g[np] = gy; A.dt_g[np] = BB_F32; A.in[np] = nd.base[0]; A.dt_in[np] = nd.dt[0]; ++np;
     if (!base && actX) { A.g[np] = nd.a[3]; A.dt_g[np] = BB_F32; A.in[np] = nd.t[0]; A.dt_in[np] = BB_F32; ++np; }
@@ -362,8 +375,6 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
       bb_launch_tally += 1;
     }
     A.out = out;
-    A.N = g.N; A.CI = g.C; A.H = g.H; A.W = g.W; A.CO = g.O; A.KH = g.KH; A.KW = g.KW; A.HO = g.HO; A.WO = g.WO;
-    A.ph = g.ph; A.pw = g.pw; A.C_orig = g.C;
     rc = small_wgrad(A, s);
     if (rc) return rc;
   } else if (need & 2) {
@@ -400,5 +411,52 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     BB_LAUNCH_CHECK();
     if (part != nullptr && (rc = bb_partials_reduce(part, gy_blocks, g.O, out, s))) return rc;
   }
+  return BB_OK;
+}
+
+// The route and geometry the small-channel launchers would choose for a stride-1 fp32 node (N, C, H, W) -> O, KHxKW,
+// padding (ph, pw), without launching anything (tests).  which: 0 tangent forward, 1 data gradient, 2 weight gradient.
+// out[15]: route (0 generic implicit GEMM, 1 corr2, 2 first-generation correlation, 3 wgrad2, 4 first-generation
+// weight gradient), grid, work units (correlation) or images per block (weight gradient), then for corr2 PX, IMGS, RY,
+// bands, CIC, nstages, VW, image groups, for wgrad2 OB, tasks, row slices, and for both weight gradients the floats of
+// one block's partial; -1 where a field does not apply.  The environment switches the launchers read are honoured.
+extern "C" int bb_conv_small_geometry(int which, int N, int CI, int H, int W, int CO, int KH, int KW, int ph, int pw,
+                                      int npairs, int64_t* out, int cap) {
+  if (cap < 15 || which < 0 || which > 2 || npairs < 1 || npairs > 2 || N < 1) return BB_ERR_ARG;
+  for (int i = 0; i < 15; ++i) out[i] = -1;
+  Geom g{};
+  g.N = N; g.C = CI; g.H = H; g.W = W; g.O = CO; g.KH = KH; g.KW = KW; g.ph = ph; g.pw = pw;
+  g.HO = H + 2 * ph - KH + 1; g.WO = W + 2 * pw - KW + 1;
+  g.sh = g.sw = g.dh = g.dw = 1;
+  if (g.HO < 1 || g.WO < 1) return BB_ERR_ARG;
+  const bool v1 = getenv("BB200_CONV_SMALL_V1") != nullptr;
+  out[0] = 0;
+  if (which < 2) {
+    SmallConvArgs A = which == 0 ? small_fwd_args(g) : small_dgrad_args(g);
+    A.npairs = npairs;
+    if (getenv("BB200_CONV_IGEMM") || !bb_conv_small_corr_ok(A.CI, A.CO, A.KH, A.KW, npairs)) return BB_OK;
+    int64_t geo[10];
+    if (!v1 && bb_conv_small_corr2_geometry(A, geo)) {
+      out[0] = 1;
+      out[1] = geo[0];
+      for (int i = 1; i < 10; ++i) out[1 + i] = geo[i];
+    } else {
+      const int64_t total = (int64_t)A.N * A.HO * ((A.WO + 3) / 4);   // conv_small.cu: PX = 4, 256 threads per block
+      out[0] = 2; out[1] = (total + 255) / 256; out[2] = total; out[3] = 4;
+    }
+    return BB_OK;
+  }
+  SmallConvArgs A = small_fwd_args(g);
+  A.npairs = npairs;
+  if (getenv("BB200_CONV_IGEMM") || !bb_conv_small_wgrad_ok(g.O, g.C, g.H, g.W, g.HO, g.WO, g.KH, g.KW)) return BB_OK;
+  int64_t geo[5];
+  if (!v1 && bb_conv_small_wgrad2_geometry(A, geo)) {
+    out[0] = 3; out[1] = geo[0];
+    out[11] = geo[1]; out[12] = geo[2]; out[13] = geo[3]; out[14] = geo[4];
+  } else {
+    bb_conv_small_wgrad_geometry(A, geo);
+    out[0] = 4; out[1] = geo[0]; out[14] = geo[1];
+  }
+  out[2] = (N + out[1] - 1) / out[1];
   return BB_OK;
 }

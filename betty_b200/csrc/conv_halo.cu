@@ -464,12 +464,51 @@ __global__ void __launch_bounds__(256) partials_reduce_kernel(const float* __res
   }
 }
 
+// Same sum for hundreds of partials of a few thousand elements.  Block = 32 elements x 32 lanes: lane l adds the
+// partials b = l, l + 32, ... in order (four loads in flight), then the lanes are added in lane order.  (One thread per
+// element walking all the partials would wait on a memory round trip per partial.)
+__global__ void __launch_bounds__(1024) partials_reduce_lanes_kernel(const float* __restrict__ part, int parts, int64_t n,
+                                                                     float* __restrict__ out) {
+  __shared__ float red[32][33];
+  const int c = threadIdx.x & 31, l = threadIdx.x >> 5;
+  const int64_t i = (int64_t)blockIdx.x * 32 + c;
+  float v = 0.f;
+  if (i < n) {
+    const float* p = part + i;
+    int b = l;
+    for (; b + 96 < parts; b += 128) {
+      const float v0 = p[(int64_t)b * n], v1 = p[(int64_t)(b + 32) * n], v2 = p[(int64_t)(b + 64) * n],
+                  v3 = p[(int64_t)(b + 96) * n];
+      v += v0;
+      v += v1;
+      v += v2;
+      v += v3;
+    }
+    for (; b < parts; b += 32) v += p[(int64_t)b * n];
+  }
+  red[l][c] = v;
+  __syncthreads();
+  if (l == 0 && i < n) {
+    float sum = red[0][c];
+#pragma unroll
+    for (int k = 1; k < 32; ++k) sum += red[k][c];
+    out[i] += sum;
+  }
+}
+
 }  // namespace
 
 int bb_partials_reduce(const float* part, int parts, int64_t n, float* out, cudaStream_t s) {
   int64_t blocks = (n + 255) / 256;
   if (blocks > 4 * BB_SM_COUNT) blocks = 4 * BB_SM_COUNT;
   partials_reduce_kernel<<<(unsigned)blocks, 256, 0, s>>>(part, parts, n, out);
+  bb_launch_tally += 1;
+  BB_LAUNCH_CHECK();
+  return BB_OK;
+}
+
+int bb_partials_reduce_lanes(const float* part, int parts, int64_t n, float* out, cudaStream_t s) {
+  partials_reduce_lanes_kernel<<<(unsigned)((n + 31) / 32), 1024, 0, s>>>(part, parts, n, out);
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
   return BB_OK;

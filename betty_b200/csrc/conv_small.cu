@@ -8,11 +8,13 @@
 //                                                               -> a_x / at_x (dual: at_y*W + a_y*t_W)
 //   conv_small_wgrad_kernel  dW[o,c,i,j] += sum_p sum_{n,y,x} g_p[n,o,y,x] * in_p[n,c,y-ph+i,x-pw+j]
 //                                                               -> at_W (dual: at_y*x + a_y*t_x)
+//        each block writes its sum over its images as one partial; the partials are added onto dW in block order
 // Same maths as conv.cu (spec: oracle/plan_interp.py tf_conv2d/bb_conv2d/tb_conv2d).
 #include "../../include/betty_b200.h"
 #include "bb_common.cuh"
 #include "conv_small.h"
 #include "plan.h"
+#include "tma.h"
 
 namespace {
 
@@ -132,12 +134,13 @@ __global__ void __launch_bounds__(256) conv_small_wgrad_kernel(const __grid_cons
     if (ns < 1) ns = 1;
   }
   float acc[TPT][KW];
-  int to[TPT], tc[TPT], ti[TPT], slice[TPT];
+  int tk[TPT], to[TPT], tc[TPT], ti[TPT], slice[TPT];
   bool live[TPT];
 #pragma unroll
   for (int u = 0; u < TPT; ++u) {
     const int t = threadIdx.x + u * blockDim.x;
     const int task = (TPT == 1) ? t % tasks : t;
+    tk[u] = task;
     slice[u] = (TPT == 1) ? t / tasks : 0;
     live[u] = (TPT == 1) ? (slice[u] < ns) : (task < tasks);
     const int tt = live[u] ? task : 0;
@@ -203,12 +206,22 @@ __global__ void __launch_bounds__(256) conv_small_wgrad_kernel(const __grid_cons
       }
     }
   }
+  // fixed-order finish: the row slices of each task are added in slice order through the staging memory, which is idle
+  // now, and the block writes its partial dW (task (o, c, i) x KW taps is dW's own layout) to A.part[blockIdx.x]
+  float* red = sm;   // [ns][tasks][KW]
+  __syncthreads();
 #pragma unroll
   for (int u = 0; u < TPT; ++u) {
     if (!live[u]) continue;
-    float* dst = A.out + (((int64_t)to[u] * C + tc[u]) * A.KH + ti[u]) * KW;
 #pragma unroll
-    for (int j = 0; j < KW; ++j) atomicAdd(dst + j, acc[u][j]);
+    for (int j = 0; j < KW; ++j) red[(slice[u] * tasks + tk[u]) * KW + j] = acc[u][j];
+  }
+  __syncthreads();
+  float* dst = A.part + (int64_t)blockIdx.x * tasks * KW;
+  for (int e = threadIdx.x; e < tasks * KW; e += blockDim.x) {
+    float v = red[e];
+    for (int sl = 1; sl < ns; ++sl) v += red[sl * tasks * KW + e];
+    dst[e] = v;
   }
 }
 
@@ -242,9 +255,11 @@ int bb_conv_small_corr(const SmallConvArgs& A, cudaStream_t s) {
   return A.KW == 3 ? launch_corr<16, 3, 16>(A, s) : launch_corr<16, 5, 16>(A, s);
 }
 
+// staging of one image (g and input planes), and at least the [ns][tasks][KW] slice sums of the finish (<= 512 x 5)
 static size_t wgrad_smem_bytes(int O, int C, int H, int W, int HO, int WO) {
   const size_t gplane = (size_t)(HO * (WO | 1)) | 1, iplane = (size_t)(H * (W | 1)) | 1;
-  return sizeof(float) * (O * gplane + C * iplane);
+  const size_t stage = sizeof(float) * (O * gplane + C * iplane), red = sizeof(float) * 512 * 5;
+  return stage > red ? stage : red;
 }
 
 bool bb_conv_small_wgrad_ok(int O, int C, int H, int W, int HO, int WO, int KH, int KW) {
@@ -253,19 +268,34 @@ bool bb_conv_small_wgrad_ok(int O, int C, int H, int W, int HO, int WO, int KH, 
   return wgrad_smem_bytes(O, C, H, W, HO, WO) <= 48 * 1024;
 }
 
+void bb_conv_small_wgrad_geometry(const SmallConvArgs& A, int64_t* geo) {
+  const int64_t n = (int64_t)A.CO * A.CI * A.KH * A.KW;
+  int grid = BB_SM_COUNT * 4;
+  if (grid > A.N) grid = A.N;
+  if (bb_reduce_ws.base != nullptr) grid = bb_reduce_ws_splits(grid, sizeof(float) * n);   // a plan never allocates
+  geo[0] = grid;
+  geo[1] = n;
+}
+
 int bb_conv_small_wgrad(const SmallConvArgs& A, cudaStream_t s) {
   const int tasks = A.CO * A.CI * A.KH;
   const size_t smem = wgrad_smem_bytes(A.CO, A.CI, A.H, A.W, A.HO, A.WO);
-  int grid = BB_SM_COUNT * 4;
-  if (grid > A.N) grid = A.N;
+  int64_t geo[2];
+  bb_conv_small_wgrad_geometry(A, geo);
+  const int grid = (int)geo[0];
+  bool owned = false;
+  SmallConvArgs B = A;
+  if ((B.part = bb_partials_acquire(sizeof(float) * grid * geo[1], s, &owned)) == nullptr) return cudaErrorMemoryAllocation;
   if (tasks <= 256) {
-    if (A.KW == 3) conv_small_wgrad_kernel<3, 1><<<grid, 256, smem, s>>>(A);
-    else conv_small_wgrad_kernel<5, 1><<<grid, 256, smem, s>>>(A);
+    if (A.KW == 3) conv_small_wgrad_kernel<3, 1><<<grid, 256, smem, s>>>(B);
+    else conv_small_wgrad_kernel<5, 1><<<grid, 256, smem, s>>>(B);
   } else {
-    if (A.KW == 3) conv_small_wgrad_kernel<3, 2><<<grid, 256, smem, s>>>(A);
-    else conv_small_wgrad_kernel<5, 2><<<grid, 256, smem, s>>>(A);
+    if (A.KW == 3) conv_small_wgrad_kernel<3, 2><<<grid, 256, smem, s>>>(B);
+    else conv_small_wgrad_kernel<5, 2><<<grid, 256, smem, s>>>(B);
   }
   bb_launch_tally += 1;
-  BB_LAUNCH_CHECK();
-  return BB_OK;
+  int rc = (int)cudaPeekAtLastError();
+  if (rc == BB_OK) rc = bb_partials_reduce_lanes(B.part, grid, geo[1], A.out, s);
+  bb_partials_release(B.part, owned, s);
+  return rc;
 }

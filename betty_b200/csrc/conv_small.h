@@ -13,6 +13,7 @@ struct SmallConvArgs {
   int npairs;
   int mode;           // corr: 0 forward indexing, 1 data-gradient indexing (transposed + flipped)
   float* out;
+  float* part;        // wgrad: per-block partials [gridDim.x][CO][CI][KH][KW] (the launcher adds them onto out in order)
   const float* bias;
   int beta;
   int N, CI, H, W, CO, KH, KW, HO, WO, ph, pw;
@@ -28,3 +29,10 @@ int bb_conv_small_wgrad(const SmallConvArgs& A, cudaStream_t s);
 // gradient; BB_DECLINED when the geometry does not fit (the callers then use the kernels above)
 int bb_conv_small_corr2(const SmallConvArgs& A, cudaStream_t s);
 int bb_conv_small_wgrad2(const SmallConvArgs& A, cudaStream_t s);
+
+// The planning of the launchers above without a launch (bb_conv_small_geometry): false when the kernel declines.
+// corr2: geo = {grid, units, PX, IMGS, RY, bands, CIC, nstages, VW, groups}
+bool bb_conv_small_corr2_geometry(const SmallConvArgs& A, int64_t* geo);
+// wgrad2: geo = {grid, OB, tasks, ns, partial floats per block};  first generation: grid and partial floats per block
+bool bb_conv_small_wgrad2_geometry(const SmallConvArgs& A, int64_t* geo);
+void bb_conv_small_wgrad_geometry(const SmallConvArgs& A, int64_t* geo);

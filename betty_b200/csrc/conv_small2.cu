@@ -13,12 +13,14 @@
 //   conv_small_wgrad2_kernel  dW[o,c,i,j] += sum_p sum_{n,y,x} g_p[n,o,y,x] * in_p[n,c,y-ph+i,x-pw+j]
 //       A thread owns (block of OB output channels, c, i) x KW taps = OB*KW accumulators; g is staged channels-last so
 //       the OB values of a pixel are one vector load, the input row slides through a register window: 2 loads per
-//       OB*KW FMAs (10:1; first generation 2.5:1).
+//       OB*KW FMAs (10:1; first generation 2.5:1).  Each block writes its sum over its images as one partial; the
+//       partials are added onto dW in block order, so the result does not depend on which block finishes first.
 #include "../../include/betty_b200.h"
 #include "bb_common.cuh"
 #include "conv_small.h"
 #include "gemm_tma.h"   // BB_DECLINED
 #include "plan.h"
+#include "tma.h"
 #include <stdlib.h>
 
 namespace {
@@ -350,14 +352,26 @@ __global__ void __launch_bounds__(256) conv_small_wgrad2_kernel(const __grid_con
     }
     if (it + 2 < items) __syncthreads();   // buffer b is refilled by the prefetch of the next iteration
   }
-  if (!live) return;
+  // fixed-order finish: the ns row slices of each task are added in slice order through the staging memory, which is
+  // idle now, and the block writes its partial dW[O][C][KH][KW] to A.part[blockIdx.x]
+  float* red = sm3;   // [ns][tasks][OB][KW]
+  __syncthreads();
+  if (live) {
 #pragma unroll
-  for (int o = 0; o < OB; ++o) {
-    const int oo = og * OB + o;
-    if (oo >= O) break;
-    float* dst = A.out + (((int64_t)oo * C + tc) * A.KH + ti) * KW;
+    for (int o = 0; o < OB; ++o)
 #pragma unroll
-    for (int j = 0; j < KW; ++j) atomicAdd(dst + j, acc[o][j]);
+      for (int j = 0; j < KW; ++j) red[((slice * G.tasks + task) * OB + o) * KW + j] = acc[o][j];
+  }
+  __syncthreads();
+  float* dst = A.part + (int64_t)blockIdx.x * O * C * A.KH * KW;
+  const int per_slice = G.tasks * OB * KW;
+  for (int e = t; e < per_slice; e += blockDim.x) {
+    const int tk = e / (OB * KW), r = e - tk * (OB * KW), o = r / KW, j = r - o * KW;
+    const int oo = (tk / (C * A.KH)) * OB + o;
+    if (oo >= O) continue;
+    float v = red[e];
+    for (int sl = 1; sl < G.ns; ++sl) v += red[sl * per_slice + e];
+    dst[(((int64_t)oo * C + (tk / A.KH) % C) * A.KH + tk % A.KH) * KW + j] = v;
   }
 }
 
@@ -426,14 +440,18 @@ bool corr2_plan(const SmallConvArgs& A, int OP, int& PX, Corr2Geom& G, size_t& s
   return false;
 }
 
+int corr2_grid(const Corr2Geom& G) {
+  const int units = G.groups * G.bands;
+  return units < BB_SM_COUNT ? units : BB_SM_COUNT;     // one persistent block per SM
+}
+
 template <int OP, int KW, int CO_T, int PX>
 int launch_corr2(const SmallConvArgs& A, const Corr2Geom& G, size_t smem, cudaStream_t s) {
   static BbOncePerDevice configured;
   if (configured.need())
     BB_CUDA_TRY(cudaFuncSetAttribute(conv_small_corr2_kernel<OP, KW, CO_T, PX>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      kCorr2SmemCap));
-  const int units = G.groups * G.bands;
-  const int grid = units < BB_SM_COUNT ? units : BB_SM_COUNT;     // one persistent block per SM
+  const int grid = corr2_grid(G);
   conv_small_corr2_kernel<OP, KW, CO_T, PX><<<grid, G.RY * 32, smem, s>>>(A, G);
   bb_launch_tally += 1;
   BB_LAUNCH_CHECK();
@@ -472,7 +490,20 @@ bool wgrad2_plan(const SmallConvArgs& A, int OB, Wgrad2Geom& G, size_t& smem) {
   G.ip = A.W | 1;
   G.iplane = (A.H * G.ip) | 1;
   smem = sizeof(float) * 2 * (((size_t)A.HO * G.gp + (size_t)C * G.iplane + 3) & ~(size_t)3);   // double buffered
+  const size_t red = sizeof(float) * (size_t)G.ns * G.tasks * OB * A.KW;   // slice sums of the finish
+  if (smem < red) smem = red;
   return smem <= (size_t)kWgrad2SmemCap;
+}
+
+int wgrad2_grid(const SmallConvArgs& A, size_t smem) {
+  int per_sm = (int)((200 * 1024) / (smem + 1024));
+  if (per_sm > 6) per_sm = 6;
+  if (per_sm < 1) per_sm = 1;
+  int grid = BB_SM_COUNT * per_sm;
+  if (grid > A.N) grid = A.N;
+  const size_t n = (size_t)A.CO * A.CI * A.KH * A.KW;
+  if (bb_reduce_ws.base != nullptr) grid = bb_reduce_ws_splits(grid, sizeof(float) * n);   // a plan never allocates
+  return grid;
 }
 
 template <int KW, int OB>
@@ -481,28 +512,56 @@ int launch_wgrad2(const SmallConvArgs& A, const Wgrad2Geom& G, size_t smem, cuda
   if (configured.need())
     BB_CUDA_TRY(cudaFuncSetAttribute(conv_small_wgrad2_kernel<KW, OB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                      kWgrad2SmemCap));
-  int per_sm = (int)((200 * 1024) / (smem + 1024));
-  if (per_sm > 6) per_sm = 6;
-  if (per_sm < 1) per_sm = 1;
-  int grid = BB_SM_COUNT * per_sm;
-  if (grid > A.N) grid = A.N;
-  conv_small_wgrad2_kernel<KW, OB><<<grid, 256, smem, s>>>(A, G);
+  const int grid = wgrad2_grid(A, smem);
+  const int64_t n = (int64_t)A.CO * A.CI * A.KH * A.KW;
+  bool owned = false;
+  SmallConvArgs B = A;
+  if ((B.part = bb_partials_acquire(sizeof(float) * grid * n, s, &owned)) == nullptr) return cudaErrorMemoryAllocation;
+  conv_small_wgrad2_kernel<KW, OB><<<grid, 256, smem, s>>>(B, G);
   bb_launch_tally += 1;
-  BB_LAUNCH_CHECK();
-  return BB_OK;
+  int rc = (int)cudaPeekAtLastError();
+  if (rc == BB_OK) rc = bb_partials_reduce_lanes(B.part, grid, n, A.out, s);
+  bb_partials_release(B.part, owned, s);
+  return rc;
 }
 
 int pick_ob(int O) { return O % 4 == 0 || O > 6 ? 4 : (O <= 2 ? 2 : 6); }
 
+bool corr2_setup(const SmallConvArgs& A, int& OP, int& PX, Corr2Geom& G, size_t& smem) {
+  if (A.CO > 16 || (A.KW != 3 && A.KW != 5) || A.HO > 512) return false;
+  OP = A.CO <= 8 ? 8 : 16;
+  return corr2_plan(A, OP, PX, G, smem);
+}
+
 }  // namespace
 
-int bb_conv_small_corr2(const SmallConvArgs& A, cudaStream_t s) {
-  if (A.CO > 16 || (A.KW != 3 && A.KW != 5) || A.HO > 512) return BB_DECLINED;
-  const int OP = A.CO <= 8 ? 8 : 16;
-  int PX = 0;
+bool bb_conv_small_corr2_geometry(const SmallConvArgs& A, int64_t* geo) {
+  int OP = 0, PX = 0;
   Corr2Geom G{};
   size_t smem = 0;
-  if (!corr2_plan(A, OP, PX, G, smem)) return BB_DECLINED;
+  if (!corr2_setup(A, OP, PX, G, smem)) return false;
+  const int64_t v[10] = {corr2_grid(G), (int64_t)G.groups * G.bands, PX, G.IMGS, G.RY, G.bands, G.CIC,
+                         (int64_t)A.npairs * ((A.CI + G.CIC - 1) / G.CIC), G.VW, G.groups};
+  for (int i = 0; i < 10; ++i) geo[i] = v[i];
+  return true;
+}
+
+bool bb_conv_small_wgrad2_geometry(const SmallConvArgs& A, int64_t* geo) {
+  if (A.KW != 3 && A.KW != 5) return false;
+  const int OB = pick_ob(A.CO);
+  Wgrad2Geom G{};
+  size_t smem = 0;
+  if (!wgrad2_plan(A, OB, G, smem)) return false;
+  const int64_t v[5] = {wgrad2_grid(A, smem), OB, G.tasks, G.ns, (int64_t)A.CO * A.CI * A.KH * A.KW};
+  for (int i = 0; i < 5; ++i) geo[i] = v[i];
+  return true;
+}
+
+int bb_conv_small_corr2(const SmallConvArgs& A, cudaStream_t s) {
+  int OP = 0, PX = 0;
+  Corr2Geom G{};
+  size_t smem = 0;
+  if (!corr2_setup(A, OP, PX, G, smem)) return BB_DECLINED;
   if (A.KW == 3) {
     if (A.CO == 6) return dispatch_px<8, 3, 6>(A, PX, G, smem, s);
     if (A.CO <= 8) return dispatch_px<8, 3, 8>(A, PX, G, smem, s);

@@ -46,6 +46,9 @@ inline int bb_reduce_ws_splits(int want, size_t per_split) {
 
 // out[i] += sum_{b < parts} part[b*n + i], b in order (the second half of a fixed-order reduction; conv_halo.cu)
 int bb_partials_reduce(const float* part, int parts, int64_t n, float* out, cudaStream_t s);
+// the same sum with each element's partials split over 32 lanes that are then added in lane order: for hundreds of
+// partials of few elements (the small-channel weight gradients, conv_small*.cu)
+int bb_partials_reduce_lanes(const float* part, int parts, int64_t n, float* out, cudaStream_t s);
 // A partial buffer of `bytes` for launcher-side reductions: the plan's workspace when it is large enough, otherwise a
 // stream-ordered allocation released by bb_partials_release (launches outside a plan, e.g. the C-ABI unit hooks).
 float* bb_partials_acquire(size_t bytes, cudaStream_t s, bool* owned);

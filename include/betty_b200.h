@@ -128,6 +128,13 @@ int bb_plan_hvp_replay(bb_plan* plan, void* stream);
 int bb_plan_invalidate_constants(bb_plan* plan);
 int bb_plan_graph_captures(const bb_plan* plan); /* how many times a K-loop iteration was captured (tests) */
 int bb_plan_node_route(bb_plan* plan, int node, int pass); /* tests: 2 = TMA tensor-core convolution path */
+/* tests: route and geometry the small-channel convolution launchers (csrc/conv_small*.cu) would choose for a stride-1
+ * fp32 conv2d node; which: 0 tangent forward, 1 data gradient, 2 weight gradient.  out[cap >= 15] = {route (0 generic,
+ * 1 corr2, 2 first-generation correlation, 3 wgrad2, 4 first-generation weight gradient), grid, work units or images
+ * per block, PX, IMGS, RY, bands, CIC, nstages, VW, image groups, OB, tasks, row slices, partial floats per block},
+ * -1 where a field does not apply.  Launches nothing. */
+int bb_conv_small_geometry(int which, int N, int CI, int H, int W, int CO, int KH, int KW, int ph, int pw, int npairs,
+                           int64_t* out, int cap);
 /* bytes of the per-node workspace of a fused data-input convolution block (BB_OP_CONVBLOCK, csrc/convblock.cu) */
 /* ---- K6 building block exposed for unit tests: halo-resident 3x3 convolution (csrc/conv_halo.cu), 64 -> 64 channels,
  *      activations bf16 in the padded NHWC layout [N][H+2][W+2][64] (zero border), weights bf16 [64][9][64] (n, tap, ch);

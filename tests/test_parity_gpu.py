@@ -66,8 +66,9 @@ def _tolerance(rec, case):
     if rec["method"] in ("neumann", "cg"):
         # 1e-4 hard.  One measured exception (tools/parity_vs_fp64.py): where the REFERENCE's
         # own fp32 result on this GPU is not reproducible to 2e-5 (lenet_cg: the conjugate-gradient steps amplify the
-        # atomics-order noise of cuDNN's backward to 3e-6 ... 1.3e-4 of the fp64 value, run to run; the engine's own
-        # atomics give it the same spread), two fp32 runs -- reference/reference as much as engine/reference -- can only
+        # atomics-order noise of cuDNN's backward to 3e-6 ... 1.3e-4 of the fp64 value, run to run; the engine's H.v is
+        # fixed-order and repeats itself bit for bit, tests/test_lenet_scale_gpu.py, so the spread is the reference's
+        # alone), two fp32 runs -- reference/reference as much as engine/reference -- can only
         # be expected within 1e-4 of the exact value EACH, i.e. within 1e-4 + the reference's measured gap of each other
         # (triangle inequality through the fp64 result).  The gap is measured here, in this process, never assumed.
         tol = 1e-4 if floor <= NOISY else 1e-4 + floor
