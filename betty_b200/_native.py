@@ -78,6 +78,7 @@ _SIGS = {
     "bb_wgrad_halo_bf16": ([C.c_int] * 4 + [C.c_void_p] * 6, 1),
     "bb_convblock_ws_bytes": ([C.c_int] * 9, 0),
     "bb_convblock2_ws_bytes": ([C.c_int] * 9, 0),
+    "bb_conv_dw_ok": ([C.c_int] * 11, 0),
     "bb_plan_neumann_loop": ([C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
                               C.c_int, C.c_void_p], None),
     "bb_plan_cg_loop": ([C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

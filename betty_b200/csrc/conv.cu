@@ -247,6 +247,26 @@ int small_wgrad(const SmallConvArgs& A, cudaStream_t s) {
   return bb_conv_small_wgrad(A, s);
 }
 
+// a_b / at_b = per-channel sum of a_y / at_y
+int bias_grad(const bb_node& nd, const Geom& g, bool base, cudaStream_t s) {
+  const void* gy = base ? nd.a[3] : nd.at[3];
+  float* out = reinterpret_cast<float*>(base ? nd.a[2] : nd.at[2]);
+  if (!nd.beta[2]) {
+    BB_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * g.O, s));
+    bb_launch_tally += 1;
+  }
+  int gy_blocks = g.N < 64 ? g.N : 64;
+  gy_blocks = bb_reduce_ws_splits(gy_blocks, sizeof(float) * g.O);     // 1 outside a plan: no partials
+  float* part = gy_blocks > 1 ? bb_reduce_ws.base : nullptr;
+  static const int small_max = getenv("BB200_CHANSUM_V1") ? 0 : 512;
+  chansum_kernel<<<dim3(g.O, gy_blocks), 256, 0, s>>>(reinterpret_cast<const float*>(gy), out, g.N, g.O, g.HO * g.WO,
+                                                      small_max, part);
+  bb_launch_tally += 1;
+  BB_LAUNCH_CHECK();
+  if (part != nullptr) return bb_partials_reduce(part, gy_blocks, g.O, out, s);
+  return BB_OK;
+}
+
 }  // namespace
 
 int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
@@ -256,9 +276,16 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
   g.sh = (int)nd.dims[9]; g.sw = (int)nd.dims[10]; g.ph = (int)nd.dims[11]; g.pw = (int)nd.dims[12];
   g.dh = (int)nd.dims[13]; g.dw = (int)nd.dims[14];
   const bool actX = nd.active & 1, actW = nd.active & 2, actB = nd.active & 4;
+  int rc;
+  if (nd.dims[15] > 1) {
+    // depthwise (groups = C = O): staged per-plane kernels for x and W, the channel sums here for the bias
+    if ((rc = bb_conv_dw_run(nd, pass, s))) return rc;
+    const bool base = pass == BB_PASS_BASE_BWD;
+    if (pass == BB_PASS_TAN_FWD || !((base ? nd.pad0 : nd.active) & 4)) return BB_OK;
+    return bias_grad(nd, g, base, s);
+  }
   const int64_t CKK = (int64_t)g.C * g.KH * g.KW, OKK = (int64_t)g.O * g.KH * g.KW;
   const int64_t P = (int64_t)g.N * g.HO * g.WO, PIN = (int64_t)g.N * g.H * g.W;
-  int rc;
   const bool unit = g.sh == 1 && g.sw == 1 && g.dh == 1 && g.dw == 1 && !getenv("BB200_CONV_IGEMM");
   const bool tc = (nd.kind & 1) && unit && !getenv("BB200_NO_TC") && g.O >= 32 && CKK <= 2048 && OKK <= 2048;
   // preferred tensor-core route: NHWC bf16 packs + TMA box loads (conv_tma.cu)
@@ -395,22 +422,7 @@ int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s) {
     rc = launch(la, lb, sc, g.O, CKK, P, np, ksplit, s);
     if (rc) return rc;
   }
-  if (need & 4) {
-    float* out = reinterpret_cast<float*>(base ? nd.a[2] : nd.at[2]);
-    if (!nd.beta[2]) {
-      BB_CUDA_TRY(cudaMemsetAsync(out, 0, sizeof(float) * g.O, s));
-      bb_launch_tally += 1;
-    }
-    int gy_blocks = g.N < 64 ? g.N : 64;
-    gy_blocks = bb_reduce_ws_splits(gy_blocks, sizeof(float) * g.O);     // 1 outside a plan: no partials
-    float* part = gy_blocks > 1 ? bb_reduce_ws.base : nullptr;
-    static const int small_max = getenv("BB200_CHANSUM_V1") ? 0 : 512;
-    chansum_kernel<<<dim3(g.O, gy_blocks), 256, 0, s>>>(reinterpret_cast<const float*>(gy), out, g.N, g.O, g.HO * g.WO,
-                                                        small_max, part);
-    bb_launch_tally += 1;
-    BB_LAUNCH_CHECK();
-    if (part != nullptr && (rc = bb_partials_reduce(part, gy_blocks, g.O, out, s))) return rc;
-  }
+  if (need & 4) return bias_grad(nd, g, base, s);
   return BB_OK;
 }
 

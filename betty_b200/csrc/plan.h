@@ -14,7 +14,7 @@ enum bb_op {
   BB_OP_MUL2 = 5,     // y = a * b
   BB_OP_SUMALL = 6,   // y = f[0] * sum(x)
   BB_OP_GEMM = 7,     // C = A.B (+ bias)               dims = M,N,K,batch
-  BB_OP_CONV2D = 8,   // NCHW direct/implicit-GEMM conv dims = N,C,H,W,O,KH,KW,HO,WO,sh,sw,ph,pw,dh,dw
+  BB_OP_CONV2D = 8,   // NCHW direct/implicit-GEMM conv dims = N,C,H,W,O,KH,KW,HO,WO,sh,sw,ph,pw,dh,dw,groups
   BB_OP_MAXPOOL2D = 9,  // gather/scatter with the base argmax (aux[0] = int64 indices) dims = NC, HW, HOWO
   BB_OP_BATCHNORM = 10, // batch statistics, NCHW       dims = N,C,HW   f[0]=eps  aux[0]=double scratch[C*16]
   BB_OP_LAYERNORM = 11, // last-dim statistics          dims = rows,D   f[0]=eps  aux[0]=float stats[rows*4]
@@ -24,6 +24,7 @@ enum bb_op {
   BB_OP_BCE_LOGITS = 15,// mean reduction               n  aux[0] = fp32 targets
   BB_OP_EMBEDDING = 16, // dims = nidx,D,V,padding_idx  aux[0] = int64 indices, aux[1] = sorted token positions + run ends (plan.py _n_embedding)
   BB_OP_AVGPOOL2D = 18, // linear: dims = NC,H,W,HO,WO,kh,kw,sh,sw,ph,pw  f[0] = 1/divisor
+                        // kind bit 0: count_include_pad=False, each window divided by its in-image taps (f[0] unused)
   BB_OP_CONVBLOCK = 19, // fused data-input conv3x3 -> BatchNorm -> [ReLU] -> MaxPool2d(2) (convblock.cu)
   BB_OP_CONVBLOCK2 = 20, // fused inner conv3x3 -> BatchNorm -> [ReLU] -> MaxPool2d(2) of a bf16 graph (convblock2.cu)
   BB_OP_DIAGSHIFT = 17, // folded c*sum((w-const)^2): at_w += f[0]*t_w over aux[0] = bb_mt_chunk[dims[0]] {a=t_w, b=at_w}
@@ -60,6 +61,8 @@ int bb_launch_ew(const bb_node& nd, int pass, cudaStream_t s);
 int bb_launch_sumall(const bb_node& nd, int pass, cudaStream_t s);
 int bb_launch_gemm(const bb_node& nd, int pass, cudaStream_t s);
 int bb_launch_conv2d(const bb_node& nd, int pass, cudaStream_t s);
+// depthwise conv2d (dims[15] = groups = C = O): input and weight terms of every pass (conv_dw.cu)
+int bb_conv_dw_run(const bb_node& nd, int pass, cudaStream_t s);
 int bb_launch_maxpool2d(const bb_node& nd, int pass, cudaStream_t s);
 int bb_launch_batchnorm(const bb_node& nd, int pass, cudaStream_t s);
 int bb_launch_layernorm(const bb_node& nd, int pass, cudaStream_t s);

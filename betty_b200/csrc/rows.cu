@@ -238,11 +238,21 @@ __global__ void __launch_bounds__(256) pool_bwd_window_kernel(float* gx, const i
   }
 }
 
-// ---- average pooling (linear; count_include_pad, floor mode) ------------------------------------------
+// ---- average pooling (linear, floor mode) -------------------------------------------------------------------------
+// exclude = 0: every window is divided by the constant divisor (inv = 1/divisor; count_include_pad or an override).
+// exclude = 1: count_include_pad=False -- each window is divided by the number of its taps inside the image.
 struct AvgGeom {
   int H, W, HO, WO, kh, kw, sh, sw, ph, pw;
   float inv;
+  int exclude;
 };
+
+// taps of output window (yo, xo) that lie inside the image
+__device__ __forceinline__ float avg_count(const AvgGeom& g, int yo, int xo) {
+  const int h0 = yo * g.sh - g.ph, w0 = xo * g.sw - g.pw;
+  const int rows = min(h0 + g.kh, g.H) - max(h0, 0), cols = min(w0 + g.kw, g.W) - max(w0, 0);
+  return (float)(rows * cols);
+}
 
 __global__ void avgpool_fwd_kernel(const float* __restrict__ tx, float* ty, int64_t nout, AvgGeom g) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -259,7 +269,7 @@ __global__ void avgpool_fwd_kernel(const float* __restrict__ tx, float* ty, int6
       if (w >= 0 && w < g.W) acc += src[h * g.W + w];
     }
   }
-  ty[i] = acc * g.inv;
+  ty[i] = g.exclude ? acc / avg_count(g, yo, xo) : acc * g.inv;
 }
 
 // gather form of the adjoint: every input pixel sums the windows that cover it (no atomics)
@@ -279,10 +289,10 @@ __global__ void avgpool_bwd_kernel(float* gx, const float* __restrict__ gy, int6
       const int ww = w + g.pw - b;
       if (ww < 0 || ww % g.sw) continue;
       const int xo = ww / g.sw;
-      if (xo < g.WO) acc += src[yo * g.WO + xo];
+      if (xo < g.WO) acc += g.exclude ? src[yo * g.WO + xo] / avg_count(g, yo, xo) : src[yo * g.WO + xo];
     }
   }
-  const float v = acc * g.inv;
+  const float v = g.exclude ? acc : acc * g.inv;
   gx[i] = beta ? gx[i] + v : v;
 }
 
@@ -412,6 +422,7 @@ int bb_launch_avgpool2d(const bb_node& nd, int pass, cudaStream_t s) {
   g.kh = (int)nd.dims[5]; g.kw = (int)nd.dims[6]; g.sh = (int)nd.dims[7]; g.sw = (int)nd.dims[8];
   g.ph = (int)nd.dims[9]; g.pw = (int)nd.dims[10];
   g.inv = (float)nd.f[0];
+  g.exclude = nd.kind & 1;
   if (pass == BB_PASS_TAN_FWD) {
     const int64_t nout = planes * g.HO * g.WO;
     if (nout <= 0) return BB_OK;

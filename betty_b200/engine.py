@@ -239,6 +239,7 @@ class HypergradientCall:
         if entry is not None:
             with _nvtx("betty_b200:prologue:rebind"):
                 if not entry.plan.rebind(tape):
+                    plan_cache.entries.pop(key, None)   # do not keep the stale plan alive next to its replacement
                     entry = None
         if entry is not None:
             plan_cache.hits += 1

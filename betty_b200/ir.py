@@ -104,6 +104,8 @@ class Graph:
     boundaries: List[Val] = field(default_factory=list)   # upper-dependent tensors entering the lower tape
     native_epilogue_ok: bool = True                        # every such tensor was captured as a boundary value
     validators: List[Any] = field(default_factory=list)    # (check() -> bool, message): data-dependent refusals
+    derived: List[Tuple[torch.Tensor, torch.Tensor]] = field(default_factory=list)  # (copy, source): contiguous
+                                                           # copies the lowering made of strided tape views
 
 
 # --------------------------------------------------------------------------------------------------
@@ -167,6 +169,7 @@ class _Lowering:
         self.boundaries: List[Val] = []
         self.native_epilogue_ok = True
         self.validators: List[Tuple[Callable[[], bool], str]] = []   # value-dependent refusals, re-checked per call
+        self.derived: List[Tuple[torch.Tensor, torch.Tensor]] = []
         self._pending_upper: set = set()
         for i, p in enumerate(tape.params):
             v = self._new(p, param_index=i, name=f"param{i}")
@@ -255,6 +258,7 @@ class _Lowering:
         g.boundaries = self.boundaries
         g.native_epilogue_ok = self.native_epilogue_ok
         g.validators = self.validators
+        g.derived = self.derived
         if fold_quadratic:
             _fold_quadratic_regularisers(g)
         _fuse_relu_maxpool(g)
@@ -320,6 +324,9 @@ class _Lowering:
                 scale = 1.0 if name.startswith("aten.sum") else 1.0 / max(1, a[0].numel())
                 self.emit("sumall", [x], op.out, name, scale=scale)
                 return
+            if name == "aten.mean.dim" and nd == 4 and sorted(d % nd for d in dims) == [2, 3] \
+                    and a[0].is_contiguous() and kw.get("dtype") is None:
+                return self._global_avgpool(op)
             raise UnsupportedGraph(f"partial reduction {name} over dims {dims}")
         if name in ("aten.mm.default", "aten.addmm.default", "aten.bmm.default", "aten.mv.default"):
             return self._gemm(op)
@@ -415,14 +422,21 @@ class _Lowering:
                 stride = stride * 2
             if len(padding) == 1:
                 padding = padding * 2
-            if ceil_mode or (not count_include_pad and any(padding)):
-                raise UnsupportedGraph("avg_pool2d with ceil_mode / count_include_pad=False and padding")
+            if ceil_mode:
+                raise UnsupportedGraph("avg_pool2d with ceil_mode")
             self.need_contig(x, name)
             if a[0].dim() != 4 or not op.out.is_contiguous():
                 raise UnsupportedGraph("avg_pool2d: only contiguous NCHW")
+            # count_include_pad=False: a window is divided by its taps inside the image (only windows that reach into
+            # the padding differ from the constant divisor); a divisor override takes precedence, as in aten
+            exclude_pad = not count_include_pad and any(padding) and not divisor
+            # (no constant divisor on such a node: a rule that ignored exclude_pad would fail instead of using k*k)
             self.emit("avgpool2d", [x], op.out, name, kernel=tuple(kernel), stride=tuple(stride), padding=tuple(padding),
-                      divisor=float(divisor) if divisor else float(kernel[0] * kernel[1]))
+                      divisor=None if exclude_pad else (float(divisor) if divisor else float(kernel[0] * kernel[1])),
+                      exclude_pad=exclude_pad)
             return
+        if name == "aten.cat.default":
+            return self._cat(op)
         if name == "aten.native_dropout.default":
             x = A(a[0])
             out, mask = op.out
@@ -556,6 +570,11 @@ class _Lowering:
         if x_t.dim() != 4:
             raise UnsupportedGraph("only 2-D convolutions")
         x, w, b = self.act(x_t), self.act(w_t), self.act(b_t) if b_t is not None else None
+        if x is not None and not x.base.is_contiguous():
+            # a strided view (e.g. x[:, :, 1:, 1:]) is gathered into a contiguous value first; the kernels take NCHW
+            src, x_t = x_t, x_t.detach().contiguous()
+            self.derived.append((x_t, src))          # refreshed from the new call's view when a cached plan is reused
+            x = self.emit("copy", [x], x_t, op.name + " (contiguous input)").out
         for v, what in ((x, "conv input"), (w, "conv weight")):
             if v is not None:
                 self.need_contig(v, what)
@@ -563,6 +582,40 @@ class _Lowering:
             raise UnsupportedGraph("conv output is not NCHW-contiguous (channels_last?)")
         self.emit("conv2d", [x, w, b], op.out, op.name, X=x_t, W=w_t, stride=tuple(stride), padding=tuple(padding),
                   dilation=tuple(dilation), groups=int(groups))
+
+    def _cat(self, op):
+        """``torch.cat``: the output is a root value and every parameter-dependent input is copied into its slice of
+        it (a ``narrow`` alias).  Slices of constant inputs are never written, so their tangents stay zero."""
+        a = op.args
+        ts = list(a[0])
+        dim = (a[1] if len(a) > 1 else 0) % op.out.dim()
+        if not op.out.is_contiguous():
+            raise UnsupportedGraph("cat: non-contiguous output")
+        out = self._new(op.out)
+        off = 0
+        for t in ts:
+            if t.dim() == 1 and t.numel() == 0:
+                continue                                  # legacy empty operand: takes no slice
+            x = self.act(t)
+            n = t.shape[dim]
+            if x is not None:
+                region = lambda u, dim=dim, off=off, n=n: u.narrow(dim, off, n)
+                self.nodes.append(Node("copy", [x], self.alias(out, region(op.out), region, full_cover=False), {},
+                                       src=op.name))
+            off += n
+
+    def _global_avgpool(self, op):
+        """``x.mean((-2, -1))`` of a contiguous NCHW tensor (global average pooling) as an ``avgpool2d`` node whose
+        window is the whole plane; without keepdim the output is a view of the pooled [N, C, 1, 1] value."""
+        x_t, out = op.args[0], op.out
+        x = self.act(x_t)
+        Nn, Cc, H, W = x_t.shape
+        keep = out.dim() == 4
+        pooled = out if keep else out.view(Nn, Cc, 1, 1)
+        attrs = dict(kernel=(H, W), stride=(H, W), padding=(0, 0), divisor=float(H * W), exclude_pad=False)
+        n = self.emit("avgpool2d", [x], pooled, op.name, **attrs)
+        if not keep:
+            self.alias(n.out, out, lambda t, shape=tuple(out.shape): t.view(shape))
 
     def _batchnorm(self, op):
         name, a = op.name, op.args

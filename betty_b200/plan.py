@@ -402,16 +402,27 @@ class HvpPlan:
     def _n_conv2d(self, n: Node, r):
         x, w, b = n.ins
         X, W = n.attrs["X"], n.attrs["W"]
-        if n.attrs["groups"] != 1:
-            raise UnsupportedGraph("grouped / depthwise convolution")
         if not X.is_contiguous() or not W.is_contiguous():
             raise UnsupportedGraph("conv operands must be NCHW-contiguous")
         Nn, Cc, H, Wd = X.shape
         O, _, KH, KW = W.shape
         _, _, HO, WO = n.out.base.shape
         (sh, sw), (ph, pw), (dh, dw) = n.attrs["stride"], n.attrs["padding"], n.attrs["dilation"]
-        r["dims"][0:15] = (Nn, Cc, H, Wd, O, KH, KW, HO, WO, sh, sw, ph, pw, dh, dw)
-        r["kind"] = int(X.dtype in (torch.bfloat16, torch.float16) or W.dtype in (torch.bfloat16, torch.float16))  # reduced-precision graph -> tensor cores allowed
+        groups = n.attrs["groups"]
+        reduced = X.dtype in (torch.bfloat16, torch.float16) or W.dtype in (torch.bfloat16, torch.float16)
+        if groups != 1:
+            if groups != Cc:
+                raise UnsupportedGraph(f"grouped convolution ({groups} groups of {Cc} channels; only depthwise "
+                                       f"groups == channels is supported)")
+            if O != Cc:
+                raise UnsupportedGraph(f"depthwise convolution with channel multiplier {O // Cc} (only 1 is supported)")
+            if reduced:
+                raise UnsupportedGraph("depthwise convolution in a bf16 / fp16 graph (only fp32 is supported)")
+            if not N.lib().bb_conv_dw_ok(Cc, O, groups, H, Wd, KH, KW, HO, WO, ph, pw):
+                raise UnsupportedGraph(f"depthwise convolution {KH}x{KW} over {H}x{Wd} planes (padding {ph}, {pw}): "
+                                       f"more taps or larger planes than the shared-memory staged kernels take")
+        r["dims"][0:16] = (Nn, Cc, H, Wd, O, KH, KW, HO, WO, sh, sw, ph, pw, dh, dw, groups)
+        r["kind"] = int(reduced)  # reduced-precision graph -> tensor cores allowed
         self._slot(r, 0, x, X)
         self._slot(r, 1, w, W)
         self._slot(r, 2, b, None)
@@ -503,7 +514,10 @@ class HvpPlan:
         _, _, HO, WO = n.out.base.shape
         (kh, kw), (sh, sw), (ph, pw) = n.attrs["kernel"], n.attrs["stride"], n.attrs["padding"]
         r["dims"][0:11] = (Nn * Cc, H, W, HO, WO, kh, kw, sh, sw, ph, pw)
-        r["f"][0] = 1.0 / n.attrs["divisor"]
+        if n.attrs.get("exclude_pad"):
+            r["kind"] = 1      # each window divided by its in-image taps (count_include_pad=False)
+        else:
+            r["f"][0] = 1.0 / n.attrs["divisor"]
         self._slot(r, 0, x, x.base)
         self._slot(r, 3, n.out, None)
 
@@ -639,8 +653,12 @@ class HvpPlan:
     # ---- reuse across calls (engine.py plan cache) ------------------------------------------------------------
     def tape_tensors(self) -> List[torch.Tensor]:
         """Every tape tensor this plan reads through a raw pointer or a recipe: bases of live values, the tensors the
-        node descriptors were built from, sources of derived constants."""
-        seen, out = set(), []
+        node descriptors were built from, sources of derived constants.  Contiguous copies the lowering made
+        (``Graph.derived``) are not tape tensors: their sources are listed instead."""
+        seen, out = {id(c) for c, _ in self.g.derived}, []
+        for _, src in self.g.derived:
+            out.append(src)
+            seen.add(id(src))
 
         def add(t):
             if isinstance(t, torch.Tensor) and id(t) not in seen:
@@ -674,10 +692,43 @@ class HvpPlan:
         valid), derived constants are recomputed, value-dependent refusals re-checked, the packs of K-loop constants
         invalidated and the base-backward pass re-run.  Returns False if some tensor cannot be located (caller then
         builds a fresh plan)."""
+        got = self.rebind_copies(new_tape)
+        if got is None:
+            return False
+        dsts, srcs, bases = got
+        with torch.no_grad():
+            if dsts:
+                torch._foreach_copy_(dsts, srcs)
+            for copy, src in self.g.derived:
+                copy.copy_(src)               # after the sources themselves were refreshed
+            for const, thunk in self._derived:
+                const.copy_(thunk())
+        for check, msg in getattr(self.g, "validators", ()):
+            if check():
+                raise UnsupportedGraph(msg)
+        self.boundary_bases = bases
+        N.call("bb_plan_invalidate_constants", self.handle)
+        self.g.loss.root.a.zero_()
+        self.buf(self.g.loss, "a").fill_(1.0)
+        self.run_pass(PASS_BB)
+        self.serves += 1
+        return True
+
+    def rebind_copies(self, new_tape):
+        """(old tensors, their new values, new boundary bases) that serve ``new_tape`` from this plan, or None when some
+        tensor the plan reads cannot be located in it."""
         from .trace import op_tensors, tensor_locator
 
         if self._locator is None:
             self._locator = tensor_locator(self.tape)
+            # views the lowering made of a tape tensor's memory (cat slices, pad interiors, pooled views of a mean):
+            # contiguous tape tensors by storage, so such a view is refreshed by copying the tensor that holds it
+            owners: dict = {}
+            for op in self.tape.ops:
+                for t in op_tensors(op):
+                    if t.is_contiguous() and t.numel() > 0:
+                        owners.setdefault(t.untyped_storage().data_ptr(), []).append(t)
+            self._owners = owners
         cache: dict = {}
 
         def new_of(t_old):
@@ -690,6 +741,18 @@ class HvpPlan:
                 lst = cache[i] = op_tensors(new_tape.ops[i])
             return lst[k]
 
+        def owner_of(t):
+            """A located contiguous tape tensor whose memory holds every element of the view ``t``."""
+            if t.numel() == 0:
+                return None
+            es = t.element_size()
+            lo = t.data_ptr()
+            hi = lo + es * (1 + sum((sz - 1) * st for sz, st in zip(t.shape, t.stride())))
+            for o in self._owners.get(t.untyped_storage().data_ptr(), ()):
+                if o.data_ptr() <= lo and hi <= o.data_ptr() + es * o.numel() and id(o) in self._locator:
+                    return o
+            return None
+
         param_ids = {id(p) for p in self.tape.params}
         dsts, srcs = [], []
         done = set()
@@ -698,7 +761,10 @@ class HvpPlan:
                 continue
             t_new = new_of(t_old)
             if t_new is None:
-                return False
+                t_old = owner_of(t_old)
+                t_new = None if t_old is None else new_of(t_old)
+            if t_new is None:
+                return None
             if t_new.data_ptr() == t_old.data_ptr():
                 continue                      # same storage both times (views of parameters, upper parameters)
             key = (t_old.data_ptr(), tuple(t_old.shape), t_old.stride())
@@ -712,23 +778,9 @@ class HvpPlan:
             if b.parent is None:
                 t_new = new_of(b.base)
                 if t_new is None:
-                    return False
+                    return None
                 bases[b.vid] = t_new          # the NEW upper graph is what the epilogue must differentiate through
-        with torch.no_grad():
-            if dsts:
-                torch._foreach_copy_(dsts, srcs)
-            for const, thunk in self._derived:
-                const.copy_(thunk())
-        for check, msg in getattr(self.g, "validators", ()):
-            if check():
-                raise UnsupportedGraph(msg)
-        self.boundary_bases = bases
-        N.call("bb_plan_invalidate_constants", self.handle)
-        self.g.loss.root.a.zero_()
-        self.buf(self.g.loss, "a").fill_(1.0)
-        self.run_pass(PASS_BB)
-        self.serves += 1
-        return True
+        return dsts, srcs, bases
 
     def profile(self, pas: int) -> np.ndarray:
         ms = np.zeros(len(self.recs), dtype=np.float32)

@@ -405,24 +405,48 @@ def _darts_lower_step(p: ShimProblem, batch):
     return F.cross_entropy(p.module(x, alphas), y)
 
 
-def darts_search(device="cpu", batch=16, c=8, cells=2, darts_alpha=0.01, seed=0):
-    """Config 4: finite-difference hypergradient through a DARTS-style supernet."""
+def _darts_l2_step(l2: float):
+    """The DARTS lower loss plus l2*||w||^2: shifts the lower Hessian by 2*l2*I (Neumann / CG parity cases)."""
+    if not l2:
+        return _darts_lower_step
+
+    def step(p: ShimProblem, batch):
+        return _darts_lower_step(p, batch) + l2 * sum((q ** 2).sum() for q in p.module.parameters())
+
+    return step
+
+
+def _darts_cfg(method, darts_alpha, K, alpha):
+    if method == "darts":
+        return ShimConfig(type="darts", darts_alpha=darts_alpha)
+    return ShimConfig(type=method, darts_alpha=darts_alpha, neumann_iterations=K, neumann_alpha=alpha,
+                      cg_iterations=K, cg_alpha=alpha)
+
+
+def darts_search(device="cpu", batch=16, c=8, cells=2, darts_alpha=0.01, method="darts", K=5, alpha=0.01, l2=0.0,
+                 seed=0):
+    """Config 4: hypergradient through a DARTS-style supernet -- finite differences (``darts``) or the implicit
+    gradient of iDARTS (``neumann`` / ``cg`` with K iterations at step ``alpha``)."""
     torch.manual_seed(seed)
     x = torch.randn(batch, 3, 32, 32)
     y = torch.randint(0, 10, (batch,))
     lower = DartsLiteNet(c, cells, 10)
     upper = ArchParams(lower.n_edges)
-    cfg = ShimConfig(type="darts", darts_alpha=darts_alpha)
-    return _pair("neural_architecture_search", lower, _darts_lower_step, upper, cfg, (x, y), device,
-                 describe=dict(batch=batch, c=c, cells=cells, method="darts"))
+    cfg = _darts_cfg(method, darts_alpha, K, alpha)
+    describe = dict(batch=batch, c=c, cells=cells, method=method)
+    if method != "darts":
+        describe.update(K=K, alpha=alpha, l2=l2)
+    return _pair("neural_architecture_search", lower, _darts_l2_step(l2), upper, cfg, (x, y), device,
+                 describe=describe)
 
 
 
 # -- config 4 at full size: the DARTS search network Network(16, 10, 8) + Architecture(4) -------------------------
 # Restated from reference ``examples/neural_architecture_search/model_search.py:129-317`` and ``operations.py:5-196``
 # (1,930,618 parameters in 1,399 tensors; tests/test_workloads_cpu.py pins the restatement to the reference's own
-# classes: same parameter list, same logits).  Only the finite-difference K4 kernels are ours on this config; the
-# two lower forward/backward passes stay on PyTorch (SURVEY.md 8d row 4).
+# classes: same parameter list, same logits).  Under ``darts`` only the finite-difference K4 kernels are ours and the
+# two lower forward/backward passes stay on PyTorch (SURVEY.md 8d row 4); under ``neumann`` / ``cg`` the K-loop runs on
+# the native plan (depthwise convolutions: csrc/conv_dw.cu).
 DARTS_PRIMITIVES = ("none", "max_pool_3x3", "avg_pool_3x3", "skip_connect", "sep_conv_3x3", "sep_conv_5x5",
                     "dil_conv_3x3", "dil_conv_5x5")
 
@@ -549,16 +573,21 @@ class DartsArchitecture(nn.Module):
         return self.alpha_reduce, self.alpha_normal
 
 
-def darts_search_full(device="cpu", batch=64, c=16, layers=8, darts_alpha=0.01, method="darts", seed=0):
-    """Config 4 as SURVEY.md 8(d) states it: Network(16,10,8) + Architecture(4), x 64x3x32x32 (train_search.py:24)."""
+def darts_search_full(device="cpu", batch=64, c=16, layers=8, darts_alpha=0.01, method="darts", K=5, alpha=0.01,
+                      l2=0.0, seed=0):
+    """Config 4 as SURVEY.md 8(d) states it: Network(16,10,8) + Architecture(4), x 64x3x32x32 (train_search.py:24).
+    ``method`` / ``K`` / ``alpha`` / ``l2`` as in ``darts_search``."""
     torch.manual_seed(seed)
     x = torch.randn(batch, 3, 32, 32)
     y = torch.randint(0, 10, (batch,))
     lower = DartsSearchNetwork(c, 10, layers)
     upper = DartsArchitecture(4)
-    cfg = ShimConfig(type=method, darts_alpha=darts_alpha)
-    return _pair("neural_architecture_search", lower, _darts_lower_step, upper, cfg, (x, y), device,
-                 describe=dict(batch=batch, c=c, layers=layers, method=method))
+    cfg = _darts_cfg(method, darts_alpha, K, alpha)
+    describe = dict(batch=batch, c=c, layers=layers, method=method)
+    if method != "darts":
+        describe.update(K=K, alpha=alpha, l2=l2)
+    return _pair("neural_architecture_search", lower, _darts_l2_step(l2), upper, cfg, (x, y), device,
+                 describe=describe)
 
 
 def attach_adam_state(wl: Workload, steps: int = 3, lr: float = 1e-2) -> Workload:

@@ -135,6 +135,9 @@ int bb_plan_node_route(bb_plan* plan, int node, int pass); /* tests: 2 = TMA ten
  * -1 where a field does not apply.  Launches nothing. */
 int bb_conv_small_geometry(int which, int N, int CI, int H, int W, int CO, int KH, int KW, int ph, int pw, int npairs,
                            int64_t* out, int cap);
+/* 1 if the staged depthwise kernels (csrc/conv_dw.cu) take a conv2d node of this shape: groups == C == O, at most 49
+ * taps, planes within their shared-memory budget; 0 otherwise.  Launches nothing. */
+int bb_conv_dw_ok(int C, int O, int groups, int H, int W, int KH, int KW, int HO, int WO, int ph, int pw);
 /* bytes of the per-node workspace of a fused data-input convolution block (BB_OP_CONVBLOCK, csrc/convblock.cu) */
 /* ---- K6 building block exposed for unit tests: halo-resident 3x3 convolution (csrc/conv_halo.cu), 64 -> 64 channels,
  *      activations bf16 in the padded NHWC layout [N][H+2][W+2][64] (zero border), weights bf16 [64][9][64] (n, tap, ch);
